@@ -224,26 +224,45 @@ __device__ __forceinline__ void long_row(int64_t rl, int64_t sl, int64_t p1,
 }
 
 // --------------------------------------------------------------------------
-// warp-stream kernel: no block barriers at all
+// gather-pipe kernel: scattered gathers, no block barriers, a gather round always in flight
 // --------------------------------------------------------------------------
-// Every WARP walks its own sequence of small tiles (kWTile merge items, the same
-// 2*row + row_ptrs[row] coordinate, so <= kWTile/2 rows and < kWTile nonzeros plus
-// the last row).  Per tile the 32 lanes stream the slab with coalesced
-// evict-first loads, gather b for 8 nonzeros each, park the products in the
-// warp's private shared-memory strip and then sum whole rows (LANES lanes per row,
-// LANES == 1: left to right = reference order).  The slab and the extents of the
-// NEXT tile are loaded into registers before the current tile is consumed, so the
-// only exposed latency is the gather itself, and 24 independent warps per SM
-// keep thousands of gathers in flight.  Nothing but __syncwarp is needed.
-constexpr int kWTile = 256;
-constexpr int kWCap = kWTile + 64 + 8;   // staged nonzeros per warp tile
+// Every WARP walks its own sequence of small tiles (the plan's `witems` merge items of the same
+// 2*row + row_ptrs[row] coordinate, so every row of a tile but the last fits the strip).  Lane l owns
+// the nonzeros p0 + l + 32 k, k < 8: coalesced evict-first slab loads, and the gathers of structured
+// matrices fall into few cache lines.  Per iteration a warp
+//   1. issues the gathers of tile B (column indices loaded one iteration earlier), together with
+//      B's values, the row pointers of B's first kGRows + 1 rows and, when beta != 0, c of those rows;
+//   2. loads the column indices of the next tile C and the extents of the tile after it;
+//   3. sums the rows of the previous tile A from its shared-memory strip -- row pointers and c come
+//      from registers, so the row phase waits for no memory while B's gathers are in flight;
+//   4. waits for B, parks its products in the strip (the only one: A is done with it).
+// Row sums: LANES lanes per row; LANES == 1 adds left to right starting from beta*c (the reference's
+// order), a row of kWideRow or more entries is summed by the whole warp (fixed tree), a last row that
+// does not fit the strip by an order-preserving strided sum.  Nothing but __syncwarp is needed.
+constexpr int kWTile = 256;             // merge items per warp tile without a plan
+constexpr int kWCap = kWTile + 64 + 8;  // staged nonzeros per warp tile
+constexpr int kWMaxItems = kWCap - 8;   // largest `witems` a plan may choose
 constexpr int kWarpsPerCta = 8;
-constexpr int kWCtasPerSm = 2;  // 128 registers: the register-resident prefetch must not spill
-constexpr int kWideRow = 64;    // LANES == 1: rows of this many entries or more are summed by the whole warp
+constexpr int kWCtasPerSm = 2;   // warp_pipe_kernel: two strips per warp
+constexpr int kGCtasPerSm = 2;   // gather_pipe_kernel: 16 warps per SM; at 3 (80 registers) it spills and is slower
+constexpr int kGRows = 64;       // rows per tile whose row pointers and c come with the prefetch
+constexpr int kWideRow = 64;     // LANES == 1: rows of this many entries or more are summed by the whole warp
+
+// Merge items per warp tile, from the matrix's average row length d: about min(56, 240 / d) rows, so
+// the nonzeros of a tile fill the 8 gather slots of every lane (256) and its rows stay below kGRows.
+// cfg2's column parts (d ~ 3): 280 items, ~56 rows, ~168 nonzeros; d = 15: 272 items, ~240 nonzeros.
+inline int64_t witems_for(int64_t num_rows, int64_t nnz)
+{
+    if (num_rows <= 0 || nnz <= 0) return kWTile;
+    const double d = (double)nnz / (double)num_rows;
+    const double rows = 240.0 / d < 56.0 ? 240.0 / d : 56.0;
+    const int64_t items = (int64_t)(rows * (kRowW + d));
+    return items < 2 * kRowW ? 2 * kRowW : (items > kWMaxItems ? kWMaxItems : items);
+}
 
 template <typename V, typename I, int LANES, bool ADVANCED, bool DOT>
-__global__ void __launch_bounds__(kWarpsPerCta * 32, kWCtasPerSm)
-    warp_stream_kernel(const int64_t* __restrict__ tiles, int64_t num_tiles, int64_t nnz,
+__global__ void __launch_bounds__(kWarpsPerCta * 32, kGCtasPerSm)
+    gather_pipe_kernel(const int64_t* __restrict__ tiles, int64_t num_tiles, int64_t nnz,
                        const I* __restrict__ row_ptrs, const I* __restrict__ col_idxs,
                        const V* __restrict__ values, const V* __restrict__ alpha_p,
                        const V* __restrict__ b, int64_t b_stride, const V* __restrict__ beta_p,
@@ -256,182 +275,193 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kWCtasPerSm)
     wait_for_block(dot);
 
     const int lane = threadIdx.x & 31;
-    const int warp = threadIdx.x >> 5;
-    V* prod = prod_all[warp];
+    V* prod = prod_all[threadIdx.x >> 5];
     V alpha = V(1), beta = V(0);
     if (ADVANCED) {
         alpha = *alpha_p;
         beta = *beta_p;
     }
+    const bool read_c = ADVANCED && beta != V(0);
     const uint64_t pol_last = policy_evict_last();
     const uint64_t pol_first = policy_evict_first();
     const int64_t W = (int64_t)gridDim.x * kWarpsPerCta;
-    int64_t t = (int64_t)blockIdx.x * kWarpsPerCta + warp;
+    int64_t t = (int64_t)blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5);
 
-    // extents of a tile: r0, p0, r1, p1 (all lanes hold them; empty past the end)
-    auto load_ext = [&](int64_t tt, int64_t (&e)[4]) {
+    // extents of a tile: rows [r0, r1), nonzeros [p0, p1); empty past the end.  Index type I: a matrix
+    // with I = int32 has fewer than 2^31 rows and nonzeros.
+    struct Ext {
+        I r0, p0, r1, p1;
+    };
+    auto load_ext = [&](int64_t tt) {
+        Ext e{0, 0, 0, 0};
         if (tt < num_tiles) {
             const longlong2 a = *reinterpret_cast<const longlong2*>(tiles + 2 * tt);
             const longlong2 bb = *reinterpret_cast<const longlong2*>(tiles + 2 * tt + 2);
-            e[0] = a.x;
-            e[1] = a.y;
-            e[2] = bb.x;
-            e[3] = bb.y;
-        } else {
-            e[0] = e[1] = e[2] = e[3] = 0;
+            e = Ext{(I)a.x, (I)a.y, (I)bb.x, (I)bb.y};
         }
+        return e;
     };
-    // Lane l owns the nonzeros p0 + l + 32 k: consecutive lanes read consecutive entries, so
-    // the slab loads are coalesced AND the gathers of structured matrices (stencils, bands:
-    // neighbouring nonzeros reference neighbouring columns) fall into few cache lines.
-    auto load_slab = [&](const int64_t (&e)[4], I (&cols)[8], V (&vals)[8]) {
+    auto load_cols = [&](const Ext& e, I (&cols)[8]) {
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
-            const int64_t idx = e[1] + lane + 32 * k;
-            const bool ok = idx < e[3];
-            cols[k] = ok ? ld_stream(col_idxs + idx, pol_first) : I(0);
-            vals[k] = ok ? ld_stream(values + idx, pol_first) : V(0);
+            const int64_t idx = (int64_t)e.p0 + lane + 32 * k;
+            cols[k] = idx < e.p1 ? ld_stream(col_idxs + idx, pol_first) : I(0);
+        }
+    };
+    // row_ptrs[r0 + j] / c[r0 + j] of a tile: j < kGRows from the lanes' prefetch registers (all lanes
+    // call these together), beyond that a load
+    auto rp_at = [&](const I (&rv)[2], const Ext& e, int j, bool ok) -> I {
+        const I v0 = __shfl_sync(0xffffffffu, rv[0], j & 31);
+        const I v1 = __shfl_sync(0xffffffffu, rv[1], j & 31);
+        if (j < 32) return v0;
+        if (j < kGRows) return v1;
+        if ((int64_t)e.r0 + j == (int64_t)e.r1) return e.p1;
+        return ok ? row_ptrs[(int64_t)e.r0 + j] : I(0);
+    };
+    auto c_at = [&](const V (&cv)[2], const Ext& e, int j, bool ok) -> V {
+        const V v0 = __shfl_sync(0xffffffffu, cv[0], j & 31);
+        const V v1 = __shfl_sync(0xffffffffu, cv[1], j & 31);
+        if (j < 32) return v0;
+        if (j < kGRows) return v1;
+        return ok ? c[((int64_t)e.r0 + j) * c_stride] : V(0);
+    };
+    // row sums of tile A: rows [r0, r0 + nrows), products in the strip at (nonzero - p0)
+    auto row_phase = [&](const Ext& e, int nrows, const I (&rv)[2], const V (&cv)[2], V& dot_acc) {
+        constexpr int kRpp = 32 / LANES;
+        const int sub = lane % LANES;
+        for (int ps = 0; ps * kRpp < nrows; ++ps) {
+            const int rloc = ps * kRpp + lane / LANES;
+            const bool rv_ok = rloc < nrows;
+            const int64_t r = (int64_t)e.r0 + rloc;
+            int64_t s = rp_at(rv, e, rloc, rv_ok);
+            int64_t en = rp_at(rv, e, rloc + 1, rv_ok);
+            V cr = V(0);
+            if (read_c) cr = c_at(cv, e, rloc, rv_ok);
+            if (!rv_ok) s = en = 0;
+            V acc = V(0);
+            const bool wide = LANES == 1 && (en - s) >= kWideRow;
+            if (LANES == 1) {
+                if (!wide) {
+                    if (read_c && rv_ok) acc = cr * beta;
+                    for (int64_t i = s; i < en; ++i) acc += prod[i - e.p0];
+                }
+            } else {
+                for (int64_t i = s + sub; i < en; i += LANES) acc += prod[i - e.p0];
+#pragma unroll
+                for (int o = LANES / 2; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+                if (read_c && rv_ok && sub == 0) acc = cr * beta + acc;
+            }
+            if (rv_ok && sub == 0 && !wide) {
+                c[r * c_stride] = acc;
+                if (DOT) dot_acc += b[r * b_stride] * acc;
+            }
+            if (LANES == 1) {
+                unsigned wm = __ballot_sync(0xffffffffu, wide);
+                while (wm) {
+                    const int src = __ffs(wm) - 1;
+                    wm &= wm - 1;
+                    const int64_t ws = __shfl_sync(0xffffffffu, s, src);
+                    const int64_t we = __shfl_sync(0xffffffffu, en, src);
+                    V part = V(0);
+                    for (int64_t i = ws + lane; i < we; i += 32) part += prod[i - e.p0];
+                    part = warp_sum(part);  // fixed tree: deterministic
+                    if (lane == src) {
+                        if (read_c) part = cr * beta + part;
+                        c[r * c_stride] = part;
+                        if (DOT) dot_acc += b[r * b_stride] * part;
+                    }
+                }
+            }
         }
     };
 
-    int64_t cur[4], nxt[4];
-    I ncols[8];
-    V nvals[8];
-    I nrp = 0;  // row pointer of row r0 + lane (first pass of the row phase)
-    load_ext(t, cur);
-    load_ext(t + W, nxt);
-    if (cur[2] > cur[0]) {
-        load_slab(cur, ncols, nvals);
-        if (lane <= cur[2] - cur[0]) nrp = row_ptrs[cur[0] + lane];
-    }
+    Ext eB = load_ext(t), eC = load_ext(t + W);
+    I cB[8];
+    load_cols(eB, cB);
+    // tile A: the one whose products sit in the strip
+    Ext eA{0, 0, 0, 0};
+    int nA = 0;
+    I rA[2] = {0, 0};
+    V cA[2] = {V(0), V(0)};
     V dot_acc = V(0);
     for (; t < num_tiles; t += W) {
-        const int64_t r0 = cur[0], p0 = cur[1], r1 = cur[2], p1 = cur[3];
-        I cols[8];
-        V vals[8];
+        // 1. gathers, values, row pointers and c of tile B
+        const bool have = eB.r1 > eB.r0;
+        V xs[8], vB[8];
+        I rB[2] = {0, 0};
+        V cvB[2] = {V(0), V(0)};
+        if (have) {
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            cols[k] = ncols[k];
-            vals[k] = nvals[k];
-        }
-        const I rp_first = nrp;
-        // ---- prefetch the next tile's slab, row pointers and the extents after it
-        int64_t nn[4];
-        load_ext(t + 2 * W, nn);
-        if (nxt[2] > nxt[0]) {
-            load_slab(nxt, ncols, nvals);
-            if (lane <= nxt[2] - nxt[0]) nrp = row_ptrs[nxt[0] + lane];
-        }
-        if (r1 > r0) {
-            const bool long_last = (p1 - p0) > kWCap;
-            const int64_t rl = r1 - 1;
-            const int64_t sl = long_last ? (int64_t)row_ptrs[rl] : p1;
-            const int64_t pend = long_last ? sl : p1;
-            const int64_t rows_end = long_last ? rl : r1;
-            // ---- gather + products: first 256 nonzeros from the prefetched registers
-            {
-                V xs[8];
-#pragma unroll
-                for (int k = 0; k < 8; ++k) {
-                    xs[k] = V(0);
-                    if (p0 + lane + 32 * k < pend)
-                        xs[k] = ld_gather(b + (int64_t)cols[k] * b_stride, pol_last);
-                }
-#pragma unroll
-                for (int k = 0; k < 8; ++k)
-                    if (p0 + lane + 32 * k < pend)
-                        prod[lane + 32 * k] = ADVANCED ? (alpha * vals[k]) * xs[k] : vals[k] * xs[k];
+            for (int k = 0; k < 8; ++k) {
+                const int64_t idx = (int64_t)eB.p0 + lane + 32 * k;
+                const bool ok = idx < eB.p1;
+                xs[k] = ok ? ld_gather(b + (int64_t)cB[k] * b_stride, pol_last) : V(0);
+                vB[k] = ok ? ld_stream(values + idx, pol_first) : V(0);
             }
-            // ---- (rare) the part of the last row beyond 256 that still fits the strip
-            for (int64_t i = p0 + 256 + lane; i < pend; i += 32) {
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+                const int64_t r = (int64_t)eB.r0 + 32 * q + lane;
+                if (r <= eB.r1) rB[q] = row_ptrs[r];
+                if (read_c && r < eB.r1) cvB[q] = c[r * c_stride];
+            }
+        }
+        // 2. column indices of tile C, extents of the tile after it
+        const Ext eD = load_ext(t + 2 * W);
+        I cC[8];
+        load_cols(eC, cC);
+        // 3. row sums of tile A while all of that is in flight
+        if (nA > 0) row_phase(eA, nA, rA, cA, dot_acc);
+        __syncwarp();
+        // 4. products of tile B into the strip
+        nA = 0;
+        if (have) {
+            const int64_t p0 = eB.p0, p1 = eB.p1;
+            const bool long_last = (p1 - p0) > kWCap;
+            const int nrows = (int)(eB.r1 - eB.r0);
+            const int64_t sl = long_last ? (int64_t)rp_at(rB, eB, nrows - 1, true) : p1;
+#pragma unroll
+            for (int k = 0; k < 8; ++k)
+                if (p0 + lane + 32 * k < p1)
+                    prod[lane + 32 * k] = ADVANCED ? (alpha * vB[k]) * xs[k] : vB[k] * xs[k];
+            // (rare) nonzeros beyond the 256 of the registers that still belong to the strip
+            for (int64_t i = p0 + 256 + lane; i < sl; i += 32) {
                 const I col = ld_stream(col_idxs + i, pol_first);
                 const V val = ld_stream(values + i, pol_first);
                 const V x = ld_gather(b + (int64_t)col * b_stride, pol_last);
                 prod[i - p0] = ADVANCED ? (alpha * val) * x : val * x;
             }
-            __syncwarp();
-            // ---- row phase: LANES lanes per row, rows_per_pass = 32 / LANES
-            constexpr int kRpp = 32 / LANES;
-            const int sub = lane % LANES;
-            const int nrows = (int)(rows_end - r0);
-            for (int ps = 0; ps * kRpp < nrows; ++ps) {
-                const int rloc = ps * kRpp + lane / LANES;
-                const bool rv = rloc < nrows;
-                int64_t s = 0, e = 0;
-                if (LANES == 1 && ps == 0) {
-                    // row pointers of the first 33 rows came with the prefetch
-                    const I nxt_rp = __shfl_down_sync(0xffffffffu, rp_first, 1);
-                    s = rp_first;
-                    e = (lane == 31) ? (rv ? (int64_t)row_ptrs[r0 + 32] : 0) : (int64_t)nxt_rp;
-                } else if (rv) {
-                    s = row_ptrs[r0 + rloc];
-                    e = row_ptrs[r0 + rloc + 1];
-                }
-                if (!rv) s = e = 0;
-                V acc = V(0);
-                // LANES == 1 plans (average row <= 32) on skewed matrices: a row of kWideRow or more
-                // entries is not left to one lane (300 dependent adds while 31 lanes idle: the Zipf
-                // twin of cfg2 spent a quarter of its time there) but summed by the whole warp below
-                const bool wide = LANES == 1 && (e - s) >= kWideRow;
-                if (LANES == 1) {
-                    if (!wide) {
-                        if (ADVANCED && rv && beta != V(0)) acc = c[(r0 + rloc) * c_stride] * beta;
-                        for (int64_t i = s; i < e; ++i) acc += prod[i - p0];
-                    }
-                } else {
-                    for (int64_t i = s + sub; i < e; i += LANES) acc += prod[i - p0];
-#pragma unroll
-                    for (int o = LANES / 2; o > 0; o >>= 1)
-                        acc += __shfl_xor_sync(0xffffffffu, acc, o);
-                    if (ADVANCED && rv && sub == 0 && beta != V(0))
-                        acc = c[(r0 + rloc) * c_stride] * beta + acc;
-                }
-                if (rv && sub == 0 && !wide) {
-                    c[(r0 + rloc) * c_stride] = acc;
-                    if (DOT) dot_acc += b[(r0 + rloc) * b_stride] * acc;
-                }
-                if (LANES == 1) {
-                    unsigned wm = __ballot_sync(0xffffffffu, wide);
-                    while (wm) {
-                        const int src = __ffs(wm) - 1;
-                        wm &= wm - 1;
-                        const int64_t ws = __shfl_sync(0xffffffffu, s, src);
-                        const int64_t we = __shfl_sync(0xffffffffu, e, src);
-                        V part = V(0);
-                        for (int64_t i = ws + lane; i < we; i += 32) part += prod[i - p0];
-                        part = warp_sum(part);  // fixed tree: deterministic
-                        if (lane == src) {
-                            if (ADVANCED && beta != V(0)) part = c[(r0 + rloc) * c_stride] * beta + part;
-                            c[(r0 + rloc) * c_stride] = part;
-                            if (DOT) dot_acc += b[(r0 + rloc) * b_stride] * part;
-                        }
-                    }
-                }
-            }
-            // ---- a last row that does not fit the strip: the whole warp sums it
+            // a last row that does not fit the strip: the whole warp sums it
             if (long_last && !(dot.skip_from > 0 && p1 - sl >= dot.skip_from)) {
+                const int64_t rl = (int64_t)eB.r1 - 1;
                 V acc = strided_row_sum<V, I, ADVANCED>(sl + lane, p1, 32, col_idxs, values, alpha, b,
                                                         b_stride, pol_first, pol_last);
                 acc = warp_sum(acc);
                 if (lane == 0) {
-                    if (ADVANCED && beta != V(0)) acc = c[rl * c_stride] * beta + acc;
+                    if (read_c) acc = c[rl * c_stride] * beta + acc;
                     c[rl * c_stride] = acc;
                     if (DOT) dot_acc += b[rl * b_stride] * acc;
                 }
             }
-            __syncwarp();
-        }
+            eA = eB;
+            nA = long_last ? nrows - 1 : nrows;
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            cur[q] = nxt[q];
-            nxt[q] = nn[q];
+            for (int q = 0; q < 2; ++q) {
+                rA[q] = rB[q];
+                cA[q] = cvB[q];
+            }
         }
+        __syncwarp();
+        eB = eC;
+        eC = eD;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) cB[k] = cC[k];
     }
+    if (nA > 0) row_phase(eA, nA, rA, cA, dot_acc);
     if (DOT) dot_epilogue(dot_acc, dot, red, &is_last);
 }
 
 // --------------------------------------------------------------------------
-// warp-stream kernel, software pipelined: the row sums of tile k-1 (shared memory only)
+// warp-pipe kernel, software pipelined: the row sums of tile k-1 (shared memory only)
 // run while the gathers of tile k and the slab loads of tile k+1 are in flight
 // --------------------------------------------------------------------------
 template <typename V, typename I, int LANES, bool ADVANCED, bool DOT>

@@ -4,10 +4,10 @@
 // Variants (every one sums a row's products in the same order, so the choice never changes a bit):
 //   kCtaRing  csr_ring.cuh   persistent CTA, bulk-copy (cp.async.bulk / UBLKCP) ring of 4 x 48 KB stages,
 //                            lane <-> row.  Matrices whose gathers are LOCAL (stencils, bands, FEM).
-//   kWarp     warp_stream    register-prefetched slabs, products parked in a 2.6 KB strip per warp: needs
-//                            almost no shared memory, so L1 (= the number of outstanding gather misses) stays
-//                            large.  Matrices with SCATTERED gathers (uniformly random columns), and small ones.
-//   kPipe     warp_pipe      the same, software pipelined (r01): local gathers on matrices too small for the ring.
+//   kWarp     gather_pipe    register-prefetched slabs, row pointers and c; the gathers of the next tile are in
+//                            flight while a warp sums the rows of the previous one, products parked in a 2.6 KB
+//                            strip per warp.  Matrices with SCATTERED gathers (uniformly random columns), small ones.
+//   kPipe     warp_pipe      the same tiles, two strips per warp: local gathers on matrices too small for the ring.
 //   kSlab     slab_kernel    base pointers without 16-byte alignment.
 // The choice is a function of the matrix (b200_csr_plan_tune_*): the locality of its gathers, measured as the
 // number of distinct 128-byte lines of b per gather instruction of the lane <-> row schedule on a sample of
@@ -35,7 +35,10 @@ constexpr int kRingCap = 3584;
 constexpr int kRingItems = kRingCap - 512;
 
 inline int64_t num_tiles_for(int64_t num_rows, int64_t nnz) { return ceildiv(kRowW * num_rows + nnz, kTile); }
-inline int64_t num_wtiles_for(int64_t num_rows, int64_t nnz) { return ceildiv(kRowW * num_rows + nnz, kWTile); }
+inline int64_t num_wtiles_for(int64_t num_rows, int64_t nnz, int64_t items = kWTile)
+{
+    return ceildiv(kRowW * num_rows + nnz, items);
+}
 inline int64_t num_rtiles_for(int64_t num_rows, int64_t nnz)
 {
     return ceildiv(kRowW * num_rows + nnz, kRingItems);
@@ -50,7 +53,8 @@ struct b200_csr_plan {
     int64_t num_tiles = 0;
     int64_t* tiles = nullptr;  // device, 2 * (num_tiles + 1): (first row, first nonzero)
     int64_t num_wtiles = 0;
-    int64_t* wtiles = nullptr;  // same for the warp-stream kernel's kWTile-item tiles
+    int64_t* wtiles = nullptr;  // same for the warp kernels' tiles of `witems` items
+    int64_t witems = 0;         // witems_for(num_rows, nnz): chosen from the average row length
     int64_t num_rtiles = 0;
     int64_t* rtiles = nullptr;  // same for the ring kernel's kRingItems-item tiles
     int lanes = 1;
@@ -144,7 +148,7 @@ inline int grid_size(const b200_ctx* ctx, Variant v, int64_t num_tiles)
     if (v == kSlab) return (int)num_tiles;
     if (v == kCtaRing) return (int)(num_tiles < ctx->num_sms ? num_tiles : ctx->num_sms);
     const int64_t need = ceildiv(num_tiles, kWarpsPerCta);
-    const int64_t cap = (int64_t)ctx->num_sms * kWCtasPerSm;
+    const int64_t cap = (int64_t)ctx->num_sms * (v == kWarp ? kGCtasPerSm : kWCtasPerSm);
     return (int)(need < cap ? need : cap);
 }
 inline int max_grid_size(const b200_ctx* ctx) { return ctx->num_sms * 4; }
@@ -182,12 +186,12 @@ b200_status launch_one(b200_ctx* ctx, Variant v, int64_t num_tiles, const int64_
             tiles, num_tiles, nnz, row_ptrs, col_idxs, values, alpha, b, b_stride, beta, c, c_stride,
             dot);
     } else if (v == kWarp) {
-        auto k = warp_stream_kernel<V, I, LANES, ADVANCED, DOT>;
+        auto k = gather_pipe_kernel<V, I, LANES, ADVANCED, DOT>;
         static bool dbg = getenv("B200_DEBUG") != nullptr;
         if (dbg) {
             int nb = 0;
             cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k, kWarpsPerCta * 32, 0);
-            fprintf(stderr, "[b200] warp_stream_kernel: %d CTAs/SM, grid %d, tiles %lld\n", nb, grid,
+            fprintf(stderr, "[b200] gather_pipe_kernel: %d CTAs/SM, grid %d, tiles %lld\n", nb, grid,
                     (long long)num_tiles);
             dbg = false;
         }

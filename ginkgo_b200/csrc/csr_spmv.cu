@@ -180,7 +180,8 @@ b200_status plan_create(b200_ctx* ctx, int64_t num_rows, int64_t nnz, const I* r
     p->num_rows = num_rows;
     p->nnz = nnz;
     p->num_tiles = num_tiles_for(num_rows, nnz);
-    p->num_wtiles = num_wtiles_for(num_rows, nnz);
+    p->witems = witems_for(num_rows, nnz);
+    p->num_wtiles = num_wtiles_for(num_rows, nnz, p->witems);
     p->num_rtiles = num_rtiles_for(num_rows, nnz);
     p->lanes = pick_lanes(num_rows, nnz);
     p->device = ctx->device;
@@ -196,7 +197,7 @@ b200_status plan_create(b200_ctx* ctx, int64_t num_rows, int64_t nnz, const I* r
     if (num_rows > 0) {
         b200_status st = fill_plan<I>(ctx, num_rows, nnz, row_ptrs, p->num_tiles, p->tiles, kTile);
         if (st == B200_OK)
-            st = fill_plan<I>(ctx, num_rows, nnz, row_ptrs, p->num_wtiles, p->wtiles, kWTile);
+            st = fill_plan<I>(ctx, num_rows, nnz, row_ptrs, p->num_wtiles, p->wtiles, p->witems);
         if (st == B200_OK)
             st = fill_plan<I>(ctx, num_rows, nnz, row_ptrs, p->num_rtiles, p->rtiles, kRingItems);
         if (st == B200_OK) st = plan_long_rows<I>(ctx, p, row_ptrs);
@@ -537,7 +538,7 @@ b200_status plan_tune(b200_ctx* ctx, b200_csr_plan* plan, int64_t num_rows, int6
                 "[b200] csr plan tuned: rows %lld nnz %lld, %.3f lines of b per gathered element -> %s, "
                 "column-blocked parts=%d\n",
                 (long long)num_rows, (long long)nnz, plan->gather_lines,
-                plan->variant == kCtaRing ? "cta_ring" : (plan->variant == kPipe ? "warp_pipe" : "warp_stream"),
+                plan->variant == kCtaRing ? "cta_ring" : (plan->variant == kPipe ? "warp_pipe" : "gather_pipe"),
                 plan->parts);
     if (st != B200_OK) set_error("csr plan tuning failed: %s", cudaGetErrorString(cudaGetLastError()));
     return st;
@@ -648,7 +649,7 @@ B200_DEF_IS_SORTED(i64, int64_t)
 #undef B200_DEF_IS_SORTED
 
 int b200_csr_plan_variant(const b200_csr_plan* plan) { return plan ? plan->variant : -1; }
-/* overrides the tuned choice (0 slab, 2 warp_stream, 4 warp_pipe, 5 cta_ring): parity tests and
+/* overrides the tuned choice (0 slab, 2 gather_pipe, 4 warp_pipe, 5 cta_ring): parity tests and
  * experiments run every variant on the same matrix; results are the same bits whatever is set */
 void b200_csr_plan_set_variant(b200_csr_plan* plan, int variant)
 {

@@ -526,7 +526,7 @@ double gkob_csr_gather_lines(void* csr)
     return v;
 }
 
-// kernel variant the tuned plan of a Csr handle uses (2 = warp_stream, 4 = warp_pipe, 5 = cta ring); -1 if
+// kernel variant the tuned plan of a Csr handle uses (2 = gather_pipe, 4 = warp_pipe, 5 = cta ring); -1 if
 // the handle is not a double/int32 or float/int32 Csr
 int gkob_csr_kernel_variant(void* csr)
 {

@@ -168,7 +168,7 @@ b200_status b200_pipe_join(b200_pipe* pipe);
         VT* c, int64_t c_stride);
 void b200_csr_plan_destroy(b200_csr_plan* plan);
 int b200_csr_plan_variant(const b200_csr_plan* plan);
-void b200_csr_plan_set_variant(b200_csr_plan* plan, int variant); /* 0 slab, 2 warp_stream, 4 warp_pipe, 5 cta_ring */
+void b200_csr_plan_set_variant(b200_csr_plan* plan, int variant); /* 0 slab, 2 gather_pipe, 4 warp_pipe, 5 cta_ring */
 void b200_csr_plan_allow_value_copy(b200_csr_plan* plan, int allow);
 double b200_csr_plan_gather_lines(const b200_csr_plan* plan); /* -1 before tune */
 int b200_csr_plan_parts(const b200_csr_plan* plan); /* > 1: a column-blocked copy is in use */

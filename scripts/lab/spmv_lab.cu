@@ -27,7 +27,39 @@ using namespace b200::csr;
         }                                                                                  \
     } while (0)
 
-static const double kPeak = 6582.5;  // MEASURED_PEAKS.json hbm_gbs
+// the device's shape, filled in by main(): SM count and SM clock from cudaDeviceProp; the HBM peak
+// (GB/s) from MEASURED_PEAKS.json ("hbm_gbs") when that file is in the working directory, else the
+// H100 SXM data sheet's 3.35 TB/s
+static int g_sms = 132;
+static double g_ghz = 1.98;
+static double kPeak = 3350.0;
+static const char* g_peak_src = "data sheet";
+
+static void init_device()
+{
+    cudaDeviceProp prop;
+    CK(cudaGetDeviceProperties(&prop, 0));
+    g_sms = prop.multiProcessorCount;
+    int khz = 0;
+    CK(cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0));
+    if (khz > 0) g_ghz = khz / 1e6;
+    if (FILE* f = fopen("MEASURED_PEAKS.json", "r")) {
+        char buf[4096];
+        const size_t n = fread(buf, 1, sizeof buf - 1, f);
+        fclose(f);
+        buf[n] = 0;
+        if (const char* k = strstr(buf, "\"hbm_gbs\"")) {
+            const char* v = strchr(k, ':');
+            const double gbs = v ? atof(v + 1) : 0.0;
+            if (gbs > 0) {
+                kPeak = gbs;
+                g_peak_src = "MEASURED_PEAKS.json";
+            }
+        }
+    }
+    printf("device %s: %d SMs, max SM clock %.3f GHz, HBM peak %.0f GB/s (%s)\n", prop.name, g_sms, g_ghz, kPeak,
+           g_peak_src);
+}
 
 // ------------------------------------------------------------------------------ generators
 __host__ __device__ inline uint64_t mix64(uint64_t z)
@@ -514,7 +546,7 @@ void group_micro()
         CK(cudaMalloc(&p, bytes));
         CK(cudaMemset(p, 1, bytes));
         for (int ctas : {2, 3, 4}) {
-            const double t = tm.ms([&] { stream_ldg<<<148 * ctas, 512>>>((const int4*)p, bytes / 16, out); });
+            const double t = tm.ms([&] { stream_ldg<<<g_sms * ctas, 512>>>((const int4*)p, bytes / 16, out); });
             printf("micro stream_ldg  LDG.128 x4 unroll, %d CTAs/SM x 512 thr: %.4f ms  %.1f GB/s (%.1f%% of copy peak)\n",
                    ctas, t, bytes / t / 1e6, 100 * bytes / t / 1e6 / kPeak);
         }
@@ -522,7 +554,7 @@ void group_micro()
             constexpr int CH = 32768, ST = 4;
             auto k = stream_bulk<CH, ST>;
             CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, CH * ST));
-            const double t = tm.ms([&] { k<<<148, 128, CH * ST>>>(p, bytes, out); });
+            const double t = tm.ms([&] { k<<<g_sms, 128, CH * ST>>>(p, bytes, out); });
             printf("micro stream_bulk 32 KB chunks x 4 stages, 1 CTA/SM: %.4f ms  %.1f GB/s (%.1f%%)\n", t,
                    bytes / t / 1e6, 100 * bytes / t / 1e6 / kPeak);
         }
@@ -530,7 +562,7 @@ void group_micro()
             constexpr int CH = 16384, ST = 6;
             auto k = stream_bulk<CH, ST>;
             CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, CH * ST));
-            const double t = tm.ms([&] { k<<<148 * 2, 128, CH * ST>>>(p, bytes, out); });
+            const double t = tm.ms([&] { k<<<g_sms * 2, 128, CH * ST>>>(p, bytes, out); });
             printf("micro stream_bulk 16 KB chunks x 6 stages, 2 CTA/SM: %.4f ms  %.1f GB/s (%.1f%%)\n", t,
                    bytes / t / 1e6, 100 * bytes / t / 1e6 / kPeak);
         }
@@ -538,7 +570,7 @@ void group_micro()
             constexpr int CH = 49152, ST = 4;
             auto k = stream_bulk<CH, ST>;
             CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, CH * ST));
-            const double t = tm.ms([&] { k<<<148, 128, CH * ST>>>(p, bytes, out); });
+            const double t = tm.ms([&] { k<<<g_sms, 128, CH * ST>>>(p, bytes, out); });
             printf("micro stream_bulk 48 KB chunks x 4 stages, 1 CTA/SM: %.4f ms  %.1f GB/s (%.1f%%)\n", t,
                    bytes / t / 1e6, 100 * bytes / t / 1e6 / kPeak);
         }
@@ -552,21 +584,24 @@ void group_micro()
         CK(cudaMalloc(&x, 10000000 * 8));
         CK(cudaMalloc(&dout, 8));
         gen_xint<<<(10000000 + 255) / 256, 256>>>(10000000, x);
-        for (int64_t M : {1250000ll, 5000000ll, 10000000ll}) {
+        // x slices of 8 / 16 / 24 MB (one column part of cfg2 is 16 MB) and the whole 80 MB; 16 / 32 / 48
+        // warps per SM in CTAs of 512 threads, 8 independent gathers per lane
+        for (int64_t M : {1000000ll, 2000000ll, 3000000ll, 10000000ll}) {
             gen_idx<<<(int)((n + 255) / 256), 256>>>(n, M, idx);
             CK(cudaDeviceSynchronize());
             auto rep = [&](const char* l, double t) {
                 printf("micro gather_ldg  %-34s x=%3lld MB: %.4f ms  %.1f G gathers/s  (150M gathers -> %.3f ms; "
-                       "%.3f gathers/clk/SM at 1.965 GHz)\n",
+                       "%.3f gathers/clk/SM at %.3f GHz)\n",
                        l, (long long)(M * 8 / 1000000), t, n / t / 1e6, 150e6 / (n / t / 1e6) / 1e6,
-                       n / t / 1e6 / 148 / 1.965);
+                       n / t / 1e6 / g_sms / g_ghz, g_ghz);
                 fflush(stdout);
             };
-            rep("U=8  2x1024 thr/SM L1 alloc", tm.ms([&] { gather_ldg<8, false><<<148 * 2, 1024>>>(idx, n, x, dout); }));
-            rep("U=8  2x1024 thr/SM no_allocate", tm.ms([&] { gather_ldg<8, true><<<148 * 2, 1024>>>(idx, n, x, dout); }));
-            rep("U=16 1x1024 thr/SM no_allocate", tm.ms([&] { gather_ldg<16, true><<<148, 1024>>>(idx, n, x, dout); }));
-            rep("U=8  1x512 thr/SM no_allocate", tm.ms([&] { gather_ldg<8, true><<<148, 512>>>(idx, n, x, dout); }));
-            rep("U=4  2x1024 thr/SM no_allocate", tm.ms([&] { gather_ldg<4, true><<<148 * 2, 1024>>>(idx, n, x, dout); }));
+            for (int ctas : {1, 2, 3}) {
+                char l[64];
+                snprintf(l, sizeof l, "U=8  %d warps/SM no_allocate", 16 * ctas);
+                rep(l, tm.ms([&] { gather_ldg<8, true><<<g_sms * ctas, 512>>>(idx, n, x, dout); }));
+            }
+            rep("U=8  32 warps/SM L1 alloc", tm.ms([&] { gather_ldg<8, false><<<g_sms * 2, 512>>>(idx, n, x, dout); }));
         }
         CK(cudaFree(idx));
         CK(cudaFree(x));
@@ -596,11 +631,11 @@ void group_l1cap()
     CK(cudaFuncSetAttribute(k16, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     for (int kb : {0, 16, 32, 48, 64, 96, 128, 160, 192}) {
         for (int thr : {512, 1024}) {
-            const double t8 = tm.ms([&] { k8<<<148, thr, (size_t)kb * 1024>>>(idx, n, x, dout); });
-            const double t16 = tm.ms([&] { k16<<<148, thr, (size_t)kb * 1024>>>(idx, n, x, dout); });
+            const double t8 = tm.ms([&] { k8<<<g_sms, thr, (size_t)kb * 1024>>>(idx, n, x, dout); });
+            const double t16 = tm.ms([&] { k16<<<g_sms, thr, (size_t)kb * 1024>>>(idx, n, x, dout); });
             printf("micro l1cap  smem %3d KB/SM, 1 CTA x %4d thr: U=8 %.4f ms %.3f gathers/clk/SM | U=16 %.4f ms %.3f "
                    "gathers/clk/SM   (x = 40 MB, no_allocate)\n",
-                   kb, thr, t8, n / t8 / 1e6 / 148 / 1.965, t16, n / t16 / 1e6 / 148 / 1.965);
+                   kb, thr, t8, n / t8 / 1e6 / g_sms / g_ghz, t16, n / t16 / 1e6 / g_sms / g_ghz);
             fflush(stdout);
         }
     }
@@ -619,11 +654,14 @@ typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void
 __device__ __forceinline__ void tma_gather4(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int r0, int r1,
                                             int r2, int r3)
 {
+    // gather4 exists from sm_100 on; group_tma4 does not launch this on an sm_90a device
+#if !defined(__CUDA_ARCH__) || __CUDA_ARCH__ >= 1000
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes"
         " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(smem_u32(dst)),
         "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
         : "memory");
+#endif
 }
 
 constexpr int kG4Warps = 8, kG4Depth = 4, kG4Slot = 128;  // bytes of shared memory per (lane, batch)
@@ -685,6 +723,12 @@ __global__ void __launch_bounds__(kG4Warps * 32, 1)
 
 void group_tma4()
 {
+    cudaDeviceProp prop;
+    CK(cudaGetDeviceProperties(&prop, 0));
+    if (prop.major < 10) {
+        printf("tma4: the TMA gather4 path needs compute capability 10.0 or later, skipped\n");
+        return;
+    }
     Timer tm;
     void* fn = nullptr;
     cudaDriverEntryPointQueryResult qres;
@@ -722,7 +766,7 @@ void group_tma4()
             gen_idx<<<(int)((n + 255) / 256), 256>>>(n, M, idx);
             CK(cudaMemset(dout, 0, 16));
             CK(cudaMemset(bad, 0, 4));
-            gather_tma4<<<148, kG4Warps * 32, smem>>>(map, idx, n, dout, bad, x);
+            gather_tma4<<<g_sms, kG4Warps * 32, smem>>>(map, idx, n, dout, bad, x);
             cudaError_t e = cudaDeviceSynchronize();
             if (e != cudaSuccess) {
                 printf("tma4: kernel failed (box rows %d): %s\n", boxrows, cudaGetErrorString(e));
@@ -733,10 +777,10 @@ void group_tma4()
             CK(cudaMemcpy(&s_tma, dout, 8, cudaMemcpyDeviceToHost));
             CK(cudaMemcpy(&hb, bad, 4, cudaMemcpyDeviceToHost));
             CK(cudaMemset(dout, 0, 16));
-            gather_ldg<8, true><<<148 * 2, 1024>>>(idx, (n / 128) * 128, x, dout);
+            gather_ldg<8, true><<<g_sms * 2, 1024>>>(idx, (n / 128) * 128, x, dout);
             CK(cudaDeviceSynchronize());
             CK(cudaMemcpy(&s_ldg, dout, 8, cudaMemcpyDeviceToHost));
-            const double t = tm.ms([&] { gather_tma4<<<148, kG4Warps * 32, smem>>>(map, idx, n, dout, nullptr, x); });
+            const double t = tm.ms([&] { gather_tma4<<<g_sms, kG4Warps * 32, smem>>>(map, idx, n, dout, nullptr, x); });
             printf("micro gather_tma4 box rows %d x=%3lld MB: %.4f ms  %.1f G gathers/s (150M -> %.3f ms)  sum %s "
                    "(tma %.0f ldg-ish %.0f) spot-check mismatches %d\n",
                    boxrows, (long long)(M * 8 / 1000000), t, n / t / 1e6, 150e6 / (n / t / 1e6) / 1e6,
@@ -827,6 +871,7 @@ int main(int argc, char** argv)
 {
     const std::string group = argc > 1 ? argv[1] : "micro";
     const std::string name = argc > 2 ? argv[2] : "cfg2";
+    init_device();
     if (group == "micro") group_micro();
     if (group == "san") group_san();
     if (group == "tma4") group_tma4();
