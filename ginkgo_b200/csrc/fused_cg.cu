@@ -175,6 +175,14 @@ __global__ void init_scalars_kernel(V* sc, int32_t* ctl, int32_t max_iters, int3
     ctl[4] = iter_first;
 }
 
+// spmv_dot on a matrix without rows: there are no tiles, so no SpMV kernel runs and writes the dot
+template <typename V>
+__global__ void empty_dot_kernel(V* dot_out, const int32_t* ctl)
+{
+    if (ctl && ctl[0] != 0) return;
+    *dot_out = V(0);
+}
+
 inline int ew_grid(const b200_ctx* ctx, int64_t n)
 {
     int64_t g = ceildiv(n, kThreads * 4);
@@ -297,7 +305,8 @@ B200_DEF_FCG(f64, double)
 B200_DEF_FCG(f32, float)
 
 /* c = A b and *dot_out = b . c in one launch (square A; b is also the dot operand).  `work`  */
-/* provides the per-CTA partials (b200_cg_fused_work_size elements); ctl may be NULL.         */
+/* provides the per-CTA partials (b200_cg_fused_work_size elements); ctl may be NULL.  With   */
+/* num_rows == 0 the dot is 0.                                                                */
 #define B200_DEF_SPMV_DOT(V, VT, I, IT)                                                          \
     b200_status b200_csr_spmv_dot_##V##_##I(                                                     \
         b200_ctx* ctx, const b200_csr_plan* plan, int64_t num_rows, int64_t num_cols,            \
@@ -308,6 +317,11 @@ B200_DEF_FCG(f32, float)
         B200_REQUIRE(plan->num_rows == num_rows && plan->nnz == nnz, "plan does not match");     \
         const b200::csr::Variant v = b200::csr::pick_variant(col_idxs, values, plan);            \
         B200_REQUIRE(v != b200::csr::kSlab, "col_idxs/values must be 32-byte aligned");          \
+        if (num_rows == 0) {                                                                     \
+            b200::fcg::empty_dot_kernel<VT><<<1, 1, 0, ctx->stream>>>(dot_out, ctl);             \
+            B200_LAUNCH_CHECK(ctx);                                                              \
+            return B200_OK;                                                                      \
+        }                                                                                        \
         b200::csr::DotArgs<VT> dot{work, ctx->counters + 1, dot_out, ctl};                       \
         return b200::csr::launch_planned<VT, IT, false, true>(                                   \
             ctx, plan, v, nnz, row_ptrs, col_idxs, values, nullptr, b, 1, nullptr, c, 1, dot);   \
