@@ -506,11 +506,14 @@ class HostSolver:
     res_kind 0 none / 1 ResidualNorm / 2 ImplicitResidualNorm, baseline 0 rhs_norm /
     1 initial_resnorm / 2 absolute, iter_first = order inside stop::Combined;
     precond_max_bs 0 = none, 1 = scalar Jacobi, k > 1 = block Jacobi (block_ptrs given, or
-    detected by find_blocks); for "ir" the preconditioner slot is the inner solver."""
+    detected by find_blocks); for "ir" the preconditioner slot is the inner solver.
+    fused: Cg's device-resident iteration (on where applicable); fused_bicgstab: Bicgstab's, opt-in.
+    used_fused tells after apply whether such a path ran."""
 
     def __init__(self, exec_, kind, A, precond_max_bs=0, block_ptrs=None, max_iters=None,
                  res_kind=1, baseline=0, reduction=1e-8, iter_first=True, krylov_dim=30, ortho=0,
-                 fused=True, check_every=16, relaxation_factor=1.0, foci=(0.0, 1.0), initial_guess="provided"):
+                 fused=True, check_every=16, relaxation_factor=1.0, foci=(0.0, 1.0), initial_guess="provided",
+                 fused_bicgstab=False):
         self.vt = A.vt
         _host().gkob_solver_params(float(relaxation_factor), float(foci[0]), float(foci[1]))
         # "ir" only: solver::initial_guess_mode of with_default_initial_guess
@@ -525,7 +528,7 @@ class HostSolver:
         self.obj = _HostObj(exec_, fn(exec_.h, {"cg": 0, "bicgstab": 1, "gmres": 2, "fcg": 3, "cgs": 4, "ir": 5, "chebyshev": 6, "pipe_cg": 7, "gcr": 8, "minres": 9, "bicg": 10}[kind], A.h,
                                       precond_max_bs, bp, nb, -1 if max_iters is None else max_iters,
                                       res_kind, baseline, reduction, int(iter_first), krylov_dim,
-                                      ortho, int(fused), check_every), (A,))
+                                      ortho, int(bool(fused)) | (2 if fused_bicgstab else 0), check_every), (A,))
 
     def apply(self, b, x):
         _hcheck(_host().gkob_apply(self.obj.h, b.h, x.h))

@@ -67,13 +67,19 @@ __global__ void plan_kernel(const I* __restrict__ row_ptrs, int64_t num_rows, in
 }
 
 // Optional fused dot product (Krylov: q = A p and p.q in one launch): every CTA
-// adds b[row]*c[row] over its rows, publishes one partial, and the CTA that
-// arrives last sums the partials in CTA order (deterministic).  `ctl`
-// (optional) is the fused solvers' control block: ctl[0] != 0 (stopped) turns
+// adds its rows' share, publishes its partial(s), and the CTA that arrives last
+// sums the partials in CTA order (deterministic).  The kernels' DOT template value:
+//   kDotNone   no dot
+//   kDotB      result = sum b[row]*c[row]  (CG: the SpMV's own input, square A)
+//   kDotW2     result = sum w[row]*c[row] for a caller-given w with one entry per row, and
+//              result2 (optional) = sum c[row]*c[row]; two partials per CTA (BiCGStab: rr.v, s.t and t.t)
+// `ctl` (optional) is the fused solvers' control block: ctl[0] != 0 (stopped) turns
 // the launch into a no-op.
+enum : int { kDotNone = 0, kDotB = 1, kDotW2 = 2 };
+
 template <typename V>
 struct DotArgs {
-    V* partials;            // one per CTA
+    V* partials;            // one per CTA (kDotW2: two)
     unsigned int* counter;  // self-resetting ticket
     V* result;
     const int32_t* ctl;
@@ -84,6 +90,28 @@ struct DotArgs {
     // owner block this launch gathers from has landed (dist.cu, b200_halo_*_staged); nullptr: no wait
     const unsigned long long* wait_flag;
     unsigned long long wait_epoch;
+    // kDotW2 only
+    const V* w;
+    V* result2;  // nullptr: the second sum is not written
+};
+
+// a thread's share of the fused dot(s); add() is called once per finished row with its c
+template <typename V, int DOT>
+struct DotAcc {
+    V s = V(0);
+    __device__ __forceinline__ void add(const DotArgs<V>&, const V* __restrict__ b, int64_t b_stride, int64_t r, V cr)
+    {
+        if (DOT) s += b[r * b_stride] * cr;
+    }
+};
+template <typename V>
+struct DotAcc<V, kDotW2> {
+    V s = V(0), s2 = V(0);
+    __device__ __forceinline__ void add(const DotArgs<V>& dot, const V* __restrict__, int64_t, int64_t r, V cr)
+    {
+        s += dot.w[r] * cr;
+        s2 += cr * cr;
+    }
 };
 
 // every CTA's thread 0 polls the flag; the barrier publishes the acquire to the block
@@ -100,13 +128,23 @@ __device__ __forceinline__ void wait_for_block(const DotArgs<V>& dot)
     __syncthreads();
 }
 
-template <typename V>
-__device__ __forceinline__ void dot_epilogue(V dot_acc, const DotArgs<V>& dot, V* red, bool* is_last)
+// THREADS: the block size when it is a compile-time constant, 0 for blockDim.x
+template <int THREADS, typename V, int DOT>
+__device__ __forceinline__ void dot_epilogue_impl(const DotAcc<V, DOT>& acc, const DotArgs<V>& dot, V* red,
+                                                  bool* is_last)
 {
     const int tid = threadIdx.x;
-    const V s = block_sum(dot_acc, red);
+    const int64_t stride = THREADS > 0 ? THREADS : (int)blockDim.x;
+    const V s = block_sum(acc.s, red);
+    V s2 = V(0);
+    if constexpr (DOT == kDotW2) s2 = block_sum(acc.s2, red);
     if (tid == 0) {
-        dot.partials[blockIdx.x] = s;
+        if constexpr (DOT == kDotW2) {
+            dot.partials[2 * blockIdx.x] = s;
+            dot.partials[2 * blockIdx.x + 1] = s2;
+        } else {
+            dot.partials[blockIdx.x] = s;
+        }
         __threadfence();
         const unsigned int ticket = atomicAdd(dot.counter, 1u);
         *is_last = (ticket == gridDim.x - 1);
@@ -114,24 +152,41 @@ __device__ __forceinline__ void dot_epilogue(V dot_acc, const DotArgs<V>& dot, V
     __syncthreads();
     if (*is_last) {
         __threadfence();
-        V t = V(0);
-        for (int64_t k = tid; k < (int64_t)gridDim.x; k += kThreads) t += __ldcg(dot.partials + k);
+        V t = V(0), t2 = V(0);
+        for (int64_t k = tid; k < (int64_t)gridDim.x; k += stride) {
+            if constexpr (DOT == kDotW2) {
+                t += __ldcg(dot.partials + 2 * k);
+                t2 += __ldcg(dot.partials + 2 * k + 1);
+            } else {
+                t += __ldcg(dot.partials + k);
+            }
+        }
         t = block_sum(t, red);
+        if constexpr (DOT == kDotW2) t2 = block_sum(t2, red);
         if (tid == 0) {
             *dot.result = t;
+            if constexpr (DOT == kDotW2)
+                if (dot.result2) *dot.result2 = t2;
             *dot.counter = 0u;
         }
     }
 }
 
+template <typename V, int DOT>
+__device__ __forceinline__ void dot_epilogue(const DotAcc<V, DOT>& acc, const DotArgs<V>& dot, V* red, bool* is_last)
+{
+    dot_epilogue_impl<kThreads>(acc, dot, red, is_last);
+}
+
 // Row phase shared by both kernels: rows [r0, rows_end) of the tile, products in
 // prod[] indexed by (nonzero - a0), row pointers from rp(r).
-template <typename V, int LANES, bool ADVANCED, bool DOT, typename RowPtr>
+template <typename V, int LANES, bool ADVANCED, int DOT, typename RowPtr>
 __device__ __forceinline__ void row_phase(int64_t r0, int64_t rows_end, int64_t a0, const V* prod,
                                           RowPtr rp, V beta, const V* __restrict__ b,
                                           int64_t b_stride, V* __restrict__ c, int64_t c_stride,
-                                          V& dot_acc, int64_t skip_from = 0)
+                                          DotAcc<V, DOT>& dot_acc, const DotArgs<V>& dot)
 {
+    const int64_t skip_from = dot.skip_from;
     constexpr int kRowsPerPass = kThreads / LANES;
     const int tid = threadIdx.x;
     const int sub = tid % LANES;
@@ -163,7 +218,7 @@ __device__ __forceinline__ void row_phase(int64_t r0, int64_t rows_end, int64_t 
         }
         if (rv && sub == 0) {
             c[r * c_stride] = acc;
-            if (DOT) dot_acc += b[r * b_stride] * acc;
+            dot_acc.add(dot, b, b_stride, r, acc);
         }
     }
 }
@@ -204,12 +259,13 @@ __device__ __forceinline__ V strided_row_sum(int64_t start, int64_t end, int64_t
 }
 
 // last row of a tile that does not fit the staging buffer: whole-CTA sum
-template <typename V, typename I, bool ADVANCED, bool DOT>
+template <typename V, typename I, bool ADVANCED, int DOT>
 __device__ __forceinline__ void long_row(int64_t rl, int64_t sl, int64_t p1,
                                          const I* __restrict__ col_idxs,
                                          const V* __restrict__ values, V alpha, V beta,
                                          const V* __restrict__ b, int64_t b_stride,
-                                         V* __restrict__ c, int64_t c_stride, V* red, V& dot_acc,
+                                         V* __restrict__ c, int64_t c_stride, V* red,
+                                         DotAcc<V, DOT>& dot_acc, const DotArgs<V>& dot,
                                          uint64_t pol_first, uint64_t pol_last)
 {
     const int tid = threadIdx.x;
@@ -219,7 +275,7 @@ __device__ __forceinline__ void long_row(int64_t rl, int64_t sl, int64_t p1,
     if (tid == 0) {
         if (ADVANCED && beta != V(0)) acc = c[rl * c_stride] * beta + acc;
         c[rl * c_stride] = acc;
-        if (DOT) dot_acc += b[rl * b_stride] * acc;
+        dot_acc.add(dot, b, b_stride, rl, acc);
     }
 }
 
@@ -260,7 +316,7 @@ inline int64_t witems_for(int64_t num_rows, int64_t nnz)
     return items < 2 * kRowW ? 2 * kRowW : (items > kWMaxItems ? kWMaxItems : items);
 }
 
-template <typename V, typename I, int LANES, bool ADVANCED, bool DOT>
+template <typename V, typename I, int LANES, bool ADVANCED, int DOT>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, kGCtasPerSm)
     gather_pipe_kernel(const int64_t* __restrict__ tiles, int64_t num_tiles, int64_t nnz,
                        const I* __restrict__ row_ptrs, const I* __restrict__ col_idxs,
@@ -326,7 +382,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kGCtasPerSm)
         return ok ? c[((int64_t)e.r0 + j) * c_stride] : V(0);
     };
     // row sums of tile A: rows [r0, r0 + nrows), products in the strip at (nonzero - p0)
-    auto row_phase = [&](const Ext& e, int nrows, const I (&rv)[2], const V (&cv)[2], V& dot_acc) {
+    auto row_phase = [&](const Ext& e, int nrows, const I (&rv)[2], const V (&cv)[2], DotAcc<V, DOT>& dot_acc) {
         constexpr int kRpp = 32 / LANES;
         const int sub = lane % LANES;
         for (int ps = 0; ps * kRpp < nrows; ++ps) {
@@ -353,7 +409,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kGCtasPerSm)
             }
             if (rv_ok && sub == 0 && !wide) {
                 c[r * c_stride] = acc;
-                if (DOT) dot_acc += b[r * b_stride] * acc;
+                dot_acc.add(dot, b, b_stride, r, acc);
             }
             if (LANES == 1) {
                 unsigned wm = __ballot_sync(0xffffffffu, wide);
@@ -368,7 +424,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kGCtasPerSm)
                     if (lane == src) {
                         if (read_c) part = cr * beta + part;
                         c[r * c_stride] = part;
-                        if (DOT) dot_acc += b[r * b_stride] * part;
+                        dot_acc.add(dot, b, b_stride, r, part);
                     }
                 }
             }
@@ -383,7 +439,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kGCtasPerSm)
     int nA = 0;
     I rA[2] = {0, 0};
     V cA[2] = {V(0), V(0)};
-    V dot_acc = V(0);
+    DotAcc<V, DOT> dot_acc;
     for (; t < num_tiles; t += W) {
         // 1. gathers, values, row pointers and c of tile B
         const bool have = eB.r1 > eB.r0;
@@ -439,7 +495,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kGCtasPerSm)
                 if (lane == 0) {
                     if (read_c) acc = c[rl * c_stride] * beta + acc;
                     c[rl * c_stride] = acc;
-                    if (DOT) dot_acc += b[rl * b_stride] * acc;
+                    dot_acc.add(dot, b, b_stride, rl, acc);
                 }
             }
             eA = eB;
@@ -464,7 +520,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kGCtasPerSm)
 // warp-pipe kernel, software pipelined: the row sums of tile k-1 (shared memory only)
 // run while the gathers of tile k and the slab loads of tile k+1 are in flight
 // --------------------------------------------------------------------------
-template <typename V, typename I, int LANES, bool ADVANCED, bool DOT>
+template <typename V, typename I, int LANES, bool ADVANCED, int DOT>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, kWCtasPerSm)
     warp_pipe_kernel(const int64_t* __restrict__ tiles, int64_t num_tiles, int64_t nnz,
                      const I* __restrict__ row_ptrs, const I* __restrict__ col_idxs,
@@ -512,7 +568,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kWCtasPerSm)
         }
     };
     // row sums of a finished tile from its strip (reads shared memory + a few row pointers)
-    auto row_phase = [&](const V* prod, int64_t r0, int64_t p0, int nrows, I rp_first, V& dot_acc) {
+    auto row_phase = [&](const V* prod, int64_t r0, int64_t p0, int nrows, I rp_first, DotAcc<V, DOT>& dot_acc) {
         constexpr int kRpp = 32 / LANES;
         const int sub = lane % LANES;
         for (int ps = 0; ps * kRpp < nrows; ++ps) {
@@ -541,7 +597,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kWCtasPerSm)
             }
             if (rv && sub == 0) {
                 c[(r0 + rloc) * c_stride] = acc;
-                if (DOT) dot_acc += b[(r0 + rloc) * b_stride] * acc;
+                dot_acc.add(dot, b, b_stride, r0 + rloc, acc);
             }
         }
     };
@@ -561,7 +617,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kWCtasPerSm)
     int prev_nrows = 0;
     I prev_rp = 0;
     int par = 0;
-    V dot_acc = V(0);
+    DotAcc<V, DOT> dot_acc;
     for (; t < num_tiles; t += W) {
         const int64_t r0 = cur[0], p0 = cur[1], r1 = cur[2], p1 = cur[3];
         const bool have = r1 > r0;
@@ -615,7 +671,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kWCtasPerSm)
                 if (lane == 0) {
                     if (ADVANCED && beta != V(0)) acc = c[rl * c_stride] * beta + acc;
                     c[rl * c_stride] = acc;
-                    if (DOT) dot_acc += b[rl * b_stride] * acc;
+                    dot_acc.add(dot, b, b_stride, rl, acc);
                 }
             }
             prev_r0 = r0;
@@ -644,7 +700,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kWCtasPerSm)
 // --------------------------------------------------------------------------
 // fallback for unaligned base pointers: one tile per CTA, ordinary loads
 // --------------------------------------------------------------------------
-template <typename V, typename I, int LANES, bool ADVANCED, bool DOT>
+template <typename V, typename I, int LANES, bool ADVANCED, int DOT>
 __global__ void __launch_bounds__(kThreads, 3)
     slab_kernel(const int64_t* __restrict__ tiles, int64_t nnz, const I* __restrict__ row_ptrs,
                 const I* __restrict__ col_idxs, const V* __restrict__ values,
@@ -659,7 +715,7 @@ __global__ void __launch_bounds__(kThreads, 3)
     if (DOT && dot.ctl && dot.ctl[0] != 0) return;
     const int64_t r0 = tiles[2 * blockIdx.x], p0 = tiles[2 * blockIdx.x + 1];
     const int64_t r1 = tiles[2 * blockIdx.x + 2], p1 = tiles[2 * blockIdx.x + 3];
-    V dot_acc = V(0);
+    DotAcc<V, DOT> dot_acc;
     if (r1 > r0) {
         const int64_t a0 = p0 & ~int64_t(7);
         V alpha = V(1), beta = V(0);
@@ -714,10 +770,10 @@ __global__ void __launch_bounds__(kThreads, 3)
         __syncthreads();
         row_phase<V, LANES, ADVANCED, DOT>(
             r0, rows_end, a0, prod, [&](int64_t r) { return (int64_t)row_ptrs[r]; }, beta, b, b_stride,
-            c, c_stride, dot_acc, dot.skip_from);
+            c, c_stride, dot_acc, dot);
         if (long_last && !(dot.skip_from > 0 && p1 - sl >= dot.skip_from))
             long_row<V, I, ADVANCED, DOT>(rl, sl, p1, col_idxs, values, alpha, beta, b, b_stride, c,
-                                          c_stride, red, dot_acc, pol_first, pol_last);
+                                          c_stride, red, dot_acc, dot, pol_first, pol_last);
     }
     if (DOT) dot_epilogue(dot_acc, dot, red, &is_last);
 }
@@ -881,16 +937,26 @@ __global__ void __launch_bounds__(256) long_rows_kernel(LongRows lr, const I* __
     }
 }
 
-// fused dot: the long rows' share of b.c, added in row order after the main kernel has written
-// the dot of all other rows
+// fused dot: the long rows' share of the dot (b.c, or w.c and c.c with w != nullptr), added in row
+// order after the main kernel has written the dot(s) of all other rows
 template <typename V>
 __global__ void long_rows_dot_fix_kernel(LongRows lr, const V* __restrict__ b, int64_t b_stride,
                                          const V* __restrict__ c, int64_t c_stride, V* result,
-                                         const int32_t* ctl)
+                                         const int32_t* ctl, const V* __restrict__ w, V* result2)
 {
     if (ctl && ctl[0] != 0) return;
     V t = *result;
-    for (int64_t k = 0; k < lr.num_rows; ++k) t += b[lr.row[k] * b_stride] * c[lr.row[k] * c_stride];
+    if (w == nullptr) {
+        for (int64_t k = 0; k < lr.num_rows; ++k) t += b[lr.row[k] * b_stride] * c[lr.row[k] * c_stride];
+    } else {
+        V t2 = result2 ? *result2 : V(0);
+        for (int64_t k = 0; k < lr.num_rows; ++k) {
+            const V cr = c[lr.row[k] * c_stride];
+            t += w[lr.row[k]] * cr;
+            t2 += cr * cr;
+        }
+        if (result2) *result2 = t2;
+    }
     *result = t;
 }
 

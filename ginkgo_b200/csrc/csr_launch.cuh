@@ -156,7 +156,7 @@ inline int max_grid_size(const b200_ctx* ctx) { return ctx->num_sms * 4; }
 // ring configuration: short rows need more consumer warps (a pass = 32 rows is one gather round
 // trip; cfg3, 7 nnz/row, is faster with 28 warps than with 16), long rows fewer (the banded twin,
 // 15 nnz/row, is faster with 16)
-template <typename V, typename I, int LANES, bool ADVANCED, bool DOT>
+template <typename V, typename I, int LANES, bool ADVANCED, int DOT>
 b200_status launch_ring_auto(b200_ctx* ctx, int64_t num_tiles, const int64_t* tiles, int64_t nnz,
                              int64_t num_rows, const I* row_ptrs, const I* col_idxs, const V* values,
                              const V* alpha, const V* b, int64_t b_stride, const V* beta, V* c,
@@ -175,7 +175,7 @@ b200_status launch_ring_auto(b200_ctx* ctx, int64_t num_tiles, const int64_t* ti
         c_stride, dot, grid);
 }
 
-template <typename V, typename I, int LANES, bool ADVANCED, bool DOT>
+template <typename V, typename I, int LANES, bool ADVANCED, int DOT>
 b200_status launch_one(b200_ctx* ctx, Variant v, int64_t num_tiles, const int64_t* tiles,
                        int64_t nnz, const I* row_ptrs, const I* col_idxs, const V* values,
                        const V* alpha, const V* b, int64_t b_stride, const V* beta, V* c,
@@ -207,7 +207,7 @@ b200_status launch_one(b200_ctx* ctx, Variant v, int64_t num_tiles, const int64_
 }
 
 // num_rows is only needed by the ring variant (row_ptrs tail of the last tile)
-template <typename V, typename I, bool ADVANCED, bool DOT>
+template <typename V, typename I, bool ADVANCED, int DOT>
 b200_status launch_slab(b200_ctx* ctx, int lanes, Variant v, int64_t num_tiles,
                         const int64_t* tiles, int64_t nnz, const I* row_ptrs, const I* col_idxs,
                         const V* values, const V* alpha, const V* b, int64_t b_stride,
@@ -248,7 +248,7 @@ b200_status launch_slab(b200_ctx* ctx, int lanes, Variant v, int64_t num_tiles,
 // disjoint rows of c, the main kernel of a skewed matrix is latency-bound on its many short rows while the
 // long-row kernel runs at the gather rate, so together they take little more than the longer of the two.  The long rows'
 // share of the fused dot is added after the join.
-template <typename V, typename I, bool ADVANCED, bool DOT>
+template <typename V, typename I, bool ADVANCED, int DOT>
 b200_status launch_planned(b200_ctx* ctx, const b200_csr_plan* plan, Variant v, int64_t nnz, const I* row_ptrs,
                            const I* col_idxs, const V* values, const V* alpha, const V* b, int64_t b_stride,
                            const V* beta, V* c, int64_t c_stride, DotArgs<V> dot = DotArgs<V>{})
@@ -292,7 +292,8 @@ b200_status launch_planned(b200_ctx* ctx, const b200_csr_plan* plan, Variant v, 
     if (DOT) {
         LongRows lr{plan->num_long,      plan->num_long_chunks, plan->long_row,     plan->long_chunk_first,
                     plan->long_chunk_row, plan->long_tickets,    plan->long_partials};
-        long_rows_dot_fix_kernel<V><<<1, 1, 0, ctx->stream>>>(lr, b, b_stride, c, c_stride, dot.result, dot.ctl);
+        long_rows_dot_fix_kernel<V><<<1, 1, 0, ctx->stream>>>(lr, b, b_stride, c, c_stride, dot.result, dot.ctl,
+                                                              DOT == kDotW2 ? dot.w : nullptr, dot.result2);
         B200_LAUNCH_CHECK(ctx);
     }
     return B200_OK;

@@ -81,31 +81,14 @@ __device__ __forceinline__ float ld_gather_na(const float* p, uint64_t pol)
 }
 
 // fused-dot epilogue for any block size (dot_epilogue of csr_kernels.cuh assumes kThreads)
-template <typename V>
-__device__ __forceinline__ void dot_epilogue_any(V dot_acc, const DotArgs<V>& dot, V* red, bool* is_last)
+template <typename V, int DOT>
+__device__ __forceinline__ void dot_epilogue_any(const DotAcc<V, DOT>& acc, const DotArgs<V>& dot, V* red,
+                                                 bool* is_last)
 {
-    const int tid = threadIdx.x;
-    const V s = block_sum(dot_acc, red);
-    if (tid == 0) {
-        dot.partials[blockIdx.x] = s;
-        __threadfence();
-        const unsigned int ticket = atomicAdd(dot.counter, 1u);
-        *is_last = (ticket == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (*is_last) {
-        __threadfence();
-        V t = V(0);
-        for (int64_t k = tid; k < (int64_t)gridDim.x; k += blockDim.x) t += __ldcg(dot.partials + k);
-        t = block_sum(t, red);
-        if (tid == 0) {
-            *dot.result = t;
-            *dot.counter = 0u;
-        }
-    }
+    dot_epilogue_impl<0>(acc, dot, red, is_last);
 }
 
-template <typename V, typename I, int LANES, bool ADVANCED, bool DOT, int NW, int KB, bool GNA, int CAP, int STAGES,
+template <typename V, typename I, int LANES, bool ADVANCED, int DOT, int NW, int KB, bool GNA, int CAP, int STAGES,
           int NP>
 __global__ void __launch_bounds__((NW + NP) * 32, 1)
     ring_kernel(const int64_t* __restrict__ tiles, int64_t num_tiles, int64_t nnz, int64_t num_rows,
@@ -138,7 +121,7 @@ __global__ void __launch_bounds__((NW + NP) * 32, 1)
 
     const int64_t G = gridDim.x;
     const uint64_t pol_first = policy_evict_first();
-    V dot_acc = V(0);
+    DotAcc<V, DOT> dot_acc;
 
     static_assert(STAGES % NP == 0, "every producer warp owns STAGES / NP stages");
     // tiles of this CTA, in order: t = blockIdx.x + j * G; tile j lives in stage j % STAGES
@@ -302,7 +285,7 @@ __global__ void __launch_bounds__((NW + NP) * 32, 1)
                     }
                     if (mine && sub == 0) {
                         c[(r0 + rloc) * c_stride] = acc;
-                        if (DOT) dot_acc += b[(r0 + rloc) * b_stride] * acc;
+                        dot_acc.add(dot, b, b_stride, r0 + rloc, acc);
                     }
                 }
                 base = (base + npass) % NW;
@@ -331,7 +314,7 @@ __global__ void __launch_bounds__((NW + NP) * 32, 1)
                     if (lane == 0) {
                         if (ADVANCED && beta != V(0)) v = c[rl * c_stride] * beta + v;
                         c[rl * c_stride] = v;
-                        if (DOT) dot_acc += b[rl * b_stride] * v;
+                        dot_acc.add(dot, b, b_stride, rl, v);
                     }
                 }
             }
@@ -355,7 +338,7 @@ b200_status set_smem_exact(K kernel, size_t bytes)
     return B200_OK;
 }
 
-template <typename V, typename I, int LANES, bool ADVANCED, bool DOT, int NW, int KB, bool GNA, int CAP, int STAGES,
+template <typename V, typename I, int LANES, bool ADVANCED, int DOT, int NW, int KB, bool GNA, int CAP, int STAGES,
           int NP>
 b200_status launch_ring(b200_ctx* ctx, int64_t num_tiles, const int64_t* tiles, int64_t nnz,
                         int64_t num_rows, const I* row_ptrs, const I* col_idxs, const V* values,

@@ -1,0 +1,332 @@
+// Fused BiCGStab iteration for sm_90a: rho / alpha / beta / gamma / omega are produced AND consumed on
+// the device, five launches per iteration, no host round trip.
+//
+// The reference drives BiCGStab from the host with about 16 launches and two blocking device->host
+// reads of the stopping flags per iteration (core/solver/bicgstab.cpp:95-233: dot, criterion check,
+// step_1, preconditioner, SpMV, dot, step_2, norm, criterion check, finalize, preconditioner, SpMV,
+// two dots, step_3).  The same recurrence, regrouped around its three global reductions (d is the
+// inverted diagonal of a scalar Jacobi preconditioner, or absent):
+//
+//   step_p     p = r + tmp (p - omega v), tmp = rho/prev_rho*alpha/omega; y = d.p     reads 4n, writes 2n
+//   spmv_dot2  v = A y  and  beta = rr.v   (SpMV epilogue)                            matrix + 3n
+//   step_s     alpha = rho/beta; s = r - alpha v; z = d.s; ||s||^2; mid check         reads 3n, writes 2n
+//   spmv_dot2  t = A z,  gamma = s.t  and  beta = t.t   (SpMV epilogue)               matrix + 3n
+//   step_xr    omega = gamma/beta; x += alpha y + omega z; r = s - omega t;
+//              rho' = rr.r; ||r||^2; swap rho / prev_rho; top-of-iteration check      reads 6n, writes 2n
+//
+// = 2 matrix + 25 n values per iteration (Identity preconditioner: 23 n, d is not read), against 36 n for
+// the reference's kernel sequence.  Element-wise arithmetic is the reference's, operation for operation
+// (reference/solver/bicgstab_kernels.cpp:63-170), so given the same scalars p, y, s, z, x, r are the bits
+// of bicgstab::step_1/2/3 + the scalar Jacobi apply.
+//
+// Stopping is the reference's: Iteration and (Implicit)ResidualNorm in the user's order with ids 1 and 2
+// (fused_common.cuh), at the top of the iteration on r (step_xr's last CTA) and again in mid-iteration on
+// s with the same iteration number (step_s's last CTA).  A stop at the mid check owes x the update of
+// bicgstab::finalize, x += alpha y: step_s writes the status into ctl[0], which turns the second SpMV
+// into a no-op, and raises ctl[5]; step_xr of the same iteration, seeing ctl[5], does only x += alpha y
+// and clears it.  step_xr always follows step_s in an iteration, so x is final before a host that polls
+// ctl between iterations can see the stop.  Once stopped and finalized every kernel is a no-op.
+//
+// Scalars  sc[16]: 0 rho, 1 prev_rho, 2 beta (rr.v, then t.t), 3 ||r||^2, 4 tau0 (baseline norm),
+//                  5 threshold = reduction_factor * tau0, 6 alpha, 7 omega, 8 gamma, 9 ||s||^2
+// Control  ctl[8] (int32): 0 stopping_status byte (0 = running), 1 iterations done, 2 max_iters (-1 none),
+//                  3 res_kind (0 none, 1 ResidualNorm, 2 ImplicitResidualNorm), 4 iter_first,
+//                  5 finalize pending (x += alpha y still owed after a stop at the mid check)
+#include "csr_launch.cuh"
+#include "fused_common.cuh"
+
+namespace b200 {
+namespace fbicgstab {
+
+using namespace fused;  // kThreads, finish_scalars, ew_grid
+
+template <typename V>
+__global__ void __launch_bounds__(kThreads)
+    step_p_kernel(int64_t n, V* __restrict__ p, const V* __restrict__ r, const V* __restrict__ v,
+                  V* __restrict__ y, const V* __restrict__ inv_diag, const V* __restrict__ sc,
+                  const int32_t* __restrict__ ctl)
+{
+    if (ctl[0] != 0) return;
+    const V rho = sc[0], prev = sc[1], alpha = sc[6], omega = sc[7];
+    const bool plain = !(prev * omega != V(0));
+    const V tmp = plain ? V(0) : rho / prev * alpha / omega;
+    for (int64_t i = blockIdx.x * (int64_t)kThreads + threadIdx.x; i < n;
+         i += (int64_t)gridDim.x * kThreads) {
+        const V ri = r[i];
+        const V pi = plain ? ri : ri + tmp * (p[i] - omega * v[i]);
+        p[i] = pi;
+        y[i] = inv_diag ? pi * inv_diag[i] : pi;
+    }
+}
+
+// K sums of one value per thread over the grid: per-CTA partials, a ticket, and the CTA that arrives last
+// adds the partials in a fixed order.  Returns true in that CTA only, whose thread 0 then holds the sums
+// in a[]; the ticket is back at 0.
+template <typename V, int K>
+__device__ __forceinline__ bool grid_sums(V (&a)[K], V* __restrict__ partials, unsigned int* counter, V* red,
+                                          bool* is_last)
+{
+    const int tid = threadIdx.x;
+#pragma unroll
+    for (int k = 0; k < K; ++k) a[k] = block_sum(a[k], red);
+    if (tid == 0) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) partials[K * blockIdx.x + k] = a[k];
+        __threadfence();
+        const unsigned int ticket = atomicAdd(counter, 1u);
+        *is_last = (ticket == gridDim.x - 1);
+    }
+    __syncthreads();
+    if (!*is_last) return false;
+    __threadfence();
+#pragma unroll
+    for (int k = 0; k < K; ++k) a[k] = V(0);
+    for (int c = tid; c < (int)gridDim.x; c += kThreads)
+#pragma unroll
+        for (int k = 0; k < K; ++k) a[k] += __ldcg(partials + K * c + k);
+#pragma unroll
+    for (int k = 0; k < K; ++k) a[k] = block_sum(a[k], red);
+    if (tid == 0) *counter = 0u;
+    return true;
+}
+
+// the mid-iteration check on s (core/solver/bicgstab.cpp:170-186), by ONE thread: the criteria of
+// finish_scalars with the iteration number and rho of the top check and ||s|| as the residual norm
+template <typename V>
+__device__ void mid_check(V ss, const V* sc, int32_t* ctl)
+{
+    const int32_t iter = ctl[1], max_iters = ctl[2], res_kind = ctl[3], iter_first = ctl[4];
+    const bool has_it = max_iters >= 0, has_res = res_kind != 0;
+    uint8_t status = 0;
+    uint8_t id = 1;
+    for (int k = 0; k < 2 && status == 0; ++k) {
+        const bool is_it = (k == 0) == (iter_first != 0);
+        if (is_it) {
+            if (!has_it) continue;
+            if (iter >= max_iters) status = (id & kIdMask) | kFinalizedMask;
+            ++id;
+        } else {
+            if (!has_res) continue;
+            const V tau = res_kind == 1 ? sqrt(ss) : sqrt(fabs(sc[0]));
+            if (tau <= sc[5]) status = kConvergedMask | (id & kIdMask) | kFinalizedMask;
+            ++id;
+        }
+    }
+    if (status != 0) {
+        ctl[0] = status;
+        ctl[5] = 1;  // bicgstab::finalize is owed: step_xr pays it
+    }
+}
+
+template <typename V>
+__global__ void __launch_bounds__(kThreads)
+    step_s_kernel(int64_t n, const V* __restrict__ r, const V* __restrict__ v, V* __restrict__ s,
+                  V* __restrict__ z, const V* __restrict__ inv_diag, V* __restrict__ sc,
+                  int32_t* __restrict__ ctl, V* __restrict__ partials, unsigned int* __restrict__ counter)
+{
+    __shared__ V red[32];
+    __shared__ bool is_last;
+    if (ctl[0] != 0) return;
+    const V beta = sc[2];
+    const bool update = beta != V(0);
+    const V alpha = update ? sc[0] / beta : V(0);
+    V a[1] = {V(0)};
+    for (int64_t i = blockIdx.x * (int64_t)kThreads + threadIdx.x; i < n;
+         i += (int64_t)gridDim.x * kThreads) {
+        const V ri = r[i];
+        const V si = update ? ri - alpha * v[i] : ri;
+        s[i] = si;
+        z[i] = inv_diag ? si * inv_diag[i] : si;
+        a[0] += si * si;
+    }
+    if (!grid_sums(a, partials, counter, red, &is_last)) return;
+    if (threadIdx.x == 0) {
+        sc[6] = alpha;
+        sc[9] = a[0];
+        mid_check(a[0], sc, ctl);
+    }
+}
+
+// INIT: r already holds b - A x; sets rr = r and computes rho = rr.r, ||r||^2 and the baseline.
+template <typename V, bool INIT>
+__global__ void __launch_bounds__(kThreads)
+    step_xr_kernel(int64_t n, V* __restrict__ x, V* __restrict__ r, const V* __restrict__ s,
+                   const V* __restrict__ t, const V* __restrict__ y, const V* __restrict__ z,
+                   V* __restrict__ rr, V* __restrict__ sc, int32_t* __restrict__ ctl,
+                   V* __restrict__ partials, unsigned int* __restrict__ counter, int baseline, V factor)
+{
+    __shared__ V red[32];
+    __shared__ bool is_last;
+    const int tid = threadIdx.x;
+    const bool pending = !INIT && ctl[5] != 0;
+    if (!INIT && !pending && ctl[0] != 0) return;
+    V a[2] = {V(0), V(0)};
+    if (pending) {
+        // bicgstab::finalize after a stop at the mid check (reference/solver/bicgstab_kernels.cpp:155-170)
+        const V alpha = sc[6];
+        for (int64_t i = blockIdx.x * (int64_t)kThreads + tid; i < n; i += (int64_t)gridDim.x * kThreads)
+            x[i] += alpha * y[i];
+    } else {
+        const V beta = sc[2];
+        const V omega = INIT ? V(0) : (beta != V(0) ? sc[8] / beta : V(0));
+        const V alpha = INIT ? V(0) : sc[6];
+        for (int64_t i = blockIdx.x * (int64_t)kThreads + tid; i < n; i += (int64_t)gridDim.x * kThreads) {
+            V ri, rri;
+            if (INIT) {
+                ri = r[i];
+                rri = ri;
+                rr[i] = ri;
+            } else {
+                x[i] += alpha * y[i] + omega * z[i];
+                ri = s[i] - omega * t[i];
+                r[i] = ri;
+                rri = rr[i];
+            }
+            a[0] += rri * ri;
+            a[1] += ri * ri;
+        }
+    }
+    // every CTA read ctl[5] and the scalars before it took its ticket: the last one may write them
+    if (!grid_sums(a, partials, counter, red, &is_last)) return;
+    if (tid == 0) {
+        if (pending) {
+            ctl[5] = 0;
+            return;
+        }
+        if (INIT) {
+            // baseline: 0 rhs_norm (sc[4] preset to ||b||), 1 initial_resnorm, 2 absolute
+            if (baseline == 1) sc[4] = sqrt(a[1]);
+            if (baseline == 2) sc[4] = V(1);
+            sc[5] = factor * sc[4];
+        } else {
+            sc[7] = sc[2] != V(0) ? sc[8] / sc[2] : V(0);
+        }
+        finish_scalars(a[0], a[1], sc, ctl);
+    }
+}
+
+template <typename V>
+__global__ void init_scalars_kernel(V* sc, int32_t* ctl, int32_t max_iters, int32_t res_kind,
+                                    int32_t iter_first)
+{
+    // rho = prev_rho = alpha = beta = gamma = omega = 1 (reference bicgstab::initialize); the INIT
+    // finish moves rho to prev_rho
+    sc[0] = V(1);
+    sc[1] = V(1);
+    sc[2] = V(1);
+    sc[3] = V(0);
+    sc[6] = V(1);
+    sc[7] = V(1);
+    sc[8] = V(1);
+    sc[9] = V(0);
+    ctl[0] = 0;
+    ctl[1] = -1;  // the INIT finish increments to 0
+    ctl[2] = max_iters;
+    ctl[3] = res_kind;
+    ctl[4] = iter_first;
+    ctl[5] = 0;
+}
+
+// spmv_dot2 on a matrix without rows: there are no tiles, so no SpMV kernel runs and writes the sums
+template <typename V>
+__global__ void empty_dot2_kernel(V* dot_out, V* dot2_out, const int32_t* ctl)
+{
+    if (ctl && ctl[0] != 0) return;
+    *dot_out = V(0);
+    if (dot2_out) *dot2_out = V(0);
+}
+
+}  // namespace fbicgstab
+}  // namespace b200
+
+extern "C" {
+
+#define B200_DEF_FBICGSTAB(V, VT)                                                                 \
+    b200_status b200_bicgstab_fused_init_##V(                                                     \
+        b200_ctx* ctx, int64_t n, const VT* r, VT* rr, VT* p, VT* v, VT* y, VT* s, VT* t, VT* z,  \
+        VT* sc, int32_t* ctl, VT* work, int64_t max_iters, int32_t res_kind, int32_t iter_first,  \
+        int32_t baseline, VT reduction_factor)                                                    \
+    {                                                                                             \
+        B200_REQUIRE(ctx && sc && ctl && work, "null argument");                                  \
+        b200::fbicgstab::init_scalars_kernel<VT><<<1, 1, 0, ctx->stream>>>(                       \
+            sc, ctl, (int32_t)(max_iters > 0x7fffffff ? 0x7fffffff : max_iters), res_kind,        \
+            iter_first);                                                                          \
+        B200_LAUNCH_CHECK(ctx);                                                                   \
+        VT* zeroed[6] = {p, v, y, s, t, z};                                                       \
+        for (VT * a : zeroed) B200_CUDA_CHECK(cudaMemsetAsync(a, 0, sizeof(VT) * n, ctx->stream)); \
+        const int grid = b200::fused::ew_grid(ctx, n);                                            \
+        b200::fbicgstab::step_xr_kernel<VT, true><<<grid, b200::fused::kThreads, 0, ctx->stream>>>( \
+            n, nullptr, const_cast<VT*>(r), nullptr, nullptr, nullptr, nullptr, rr, sc, ctl,      \
+            work + (int64_t)ctx->num_sms * 4, ctx->counters + 2, baseline, reduction_factor);     \
+        B200_LAUNCH_CHECK(ctx);                                                                   \
+        return B200_OK;                                                                           \
+    }                                                                                             \
+    b200_status b200_bicgstab_fused_step_p_##V(b200_ctx* ctx, int64_t n, VT* p, const VT* r,      \
+                                               const VT* v, VT* y, const VT* inv_diag,            \
+                                               const VT* sc, const int32_t* ctl)                  \
+    {                                                                                             \
+        const int grid = b200::fused::ew_grid(ctx, n);                                            \
+        b200::fbicgstab::step_p_kernel<VT><<<grid, b200::fused::kThreads, 0, ctx->stream>>>(      \
+            n, p, r, v, y, inv_diag, sc, ctl);                                                    \
+        B200_LAUNCH_CHECK(ctx);                                                                   \
+        return B200_OK;                                                                           \
+    }                                                                                             \
+    b200_status b200_bicgstab_fused_step_s_##V(b200_ctx* ctx, int64_t n, const VT* r,             \
+                                               const VT* v, VT* s, VT* z, const VT* inv_diag,     \
+                                               VT* sc, int32_t* ctl, VT* work)                    \
+    {                                                                                             \
+        const int grid = b200::fused::ew_grid(ctx, n);                                            \
+        b200::fbicgstab::step_s_kernel<VT><<<grid, b200::fused::kThreads, 0, ctx->stream>>>(      \
+            n, r, v, s, z, inv_diag, sc, ctl, work + (int64_t)ctx->num_sms * 4,                   \
+            ctx->counters + 2);                                                                   \
+        B200_LAUNCH_CHECK(ctx);                                                                   \
+        return B200_OK;                                                                           \
+    }                                                                                             \
+    b200_status b200_bicgstab_fused_step_xr_##V(b200_ctx* ctx, int64_t n, VT* x, VT* r,           \
+                                                const VT* s, const VT* t, const VT* y,            \
+                                                const VT* z, const VT* rr, VT* sc, int32_t* ctl,  \
+                                                VT* work)                                         \
+    {                                                                                             \
+        const int grid = b200::fused::ew_grid(ctx, n);                                            \
+        b200::fbicgstab::step_xr_kernel<VT, false><<<grid, b200::fused::kThreads, 0,              \
+                                                     ctx->stream>>>(                              \
+            n, x, r, s, t, y, z, const_cast<VT*>(rr), sc, ctl, work + (int64_t)ctx->num_sms * 4,  \
+            ctx->counters + 2, 0, VT(0));                                                         \
+        B200_LAUNCH_CHECK(ctx);                                                                   \
+        return B200_OK;                                                                           \
+    }
+
+B200_DEF_FBICGSTAB(f64, double)
+B200_DEF_FBICGSTAB(f32, float)
+
+/* c = A b, *dot_out = w . c and (dot2_out != NULL) *dot2_out = c . c in one launch; w has one     */
+/* entry per row.  `work` and `ctl` as for b200_csr_spmv_dot_*.  With num_rows == 0 both are 0.    */
+#define B200_DEF_SPMV_DOT2(V, VT, I, IT)                                                          \
+    b200_status b200_csr_spmv_dot2_##V##_##I(                                                     \
+        b200_ctx* ctx, const b200_csr_plan* plan, int64_t num_rows, int64_t num_cols,             \
+        int64_t nnz, const IT* row_ptrs, const IT* col_idxs, const VT* values, const VT* b,       \
+        VT* c, const VT* w, VT* dot_out, VT* dot2_out, VT* work, const int32_t* ctl)              \
+    {                                                                                             \
+        B200_REQUIRE(ctx && plan && w && dot_out && work, "null argument (a plan is required)");  \
+        B200_REQUIRE(plan->num_rows == num_rows && plan->nnz == nnz, "plan does not match");      \
+        const b200::csr::Variant v = b200::csr::pick_variant(col_idxs, values, plan);             \
+        B200_REQUIRE(v != b200::csr::kSlab, "col_idxs/values must be 32-byte aligned");           \
+        if (num_rows == 0) {                                                                      \
+            b200::fbicgstab::empty_dot2_kernel<VT><<<1, 1, 0, ctx->stream>>>(dot_out, dot2_out,   \
+                                                                             ctl);                \
+            B200_LAUNCH_CHECK(ctx);                                                               \
+            return B200_OK;                                                                       \
+        }                                                                                         \
+        b200::csr::DotArgs<VT> dot{work, ctx->counters + 1, dot_out, ctl};                        \
+        dot.w = w;                                                                                \
+        dot.result2 = dot2_out;                                                                   \
+        return b200::csr::launch_planned<VT, IT, false, b200::csr::kDotW2>(                       \
+            ctx, plan, v, nnz, row_ptrs, col_idxs, values, nullptr, b, 1, nullptr, c, 1, dot);    \
+    }
+
+B200_DEF_SPMV_DOT2(f64, double, i32, int32_t)
+B200_DEF_SPMV_DOT2(f64, double, i64, int64_t)
+B200_DEF_SPMV_DOT2(f32, float, i32, int32_t)
+B200_DEF_SPMV_DOT2(f32, float, i64, int64_t)
+
+}  // extern "C"

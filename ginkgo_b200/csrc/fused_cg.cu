@@ -26,11 +26,12 @@
 //                 2 max_iters (-1 none), 3 res_kind (0 none, 1 ResidualNorm,
 //                 2 ImplicitResidualNorm), 4 iter_first
 #include "csr_launch.cuh"
+#include "fused_common.cuh"
 
 namespace b200 {
 namespace fcg {
 
-constexpr int kThreads = 512;
+using namespace fused;  // kThreads, finish_scalars, ew_grid
 
 template <typename V>
 __global__ void __launch_bounds__(kThreads)
@@ -46,35 +47,6 @@ __global__ void __launch_bounds__(kThreads)
         const V zi = z[i];
         p[i] = plain ? zi : zi + beta * p[i];
     }
-}
-
-// the reference's criteria, evaluated by ONE thread (core/stop/combined.cpp:33-52)
-template <typename V>
-__device__ void finish_scalars(V rho_new, V rr, V* sc, int32_t* ctl)
-{
-    sc[1] = sc[0];
-    sc[0] = rho_new;
-    sc[3] = rr;
-    const int32_t iter = ctl[1] + 1;
-    ctl[1] = iter;
-    const int32_t max_iters = ctl[2], res_kind = ctl[3], iter_first = ctl[4];
-    const bool has_it = max_iters >= 0, has_res = res_kind != 0;
-    uint8_t status = 0;
-    uint8_t id = 1;
-    for (int k = 0; k < 2 && status == 0; ++k) {
-        const bool is_it = (k == 0) == (iter_first != 0);
-        if (is_it) {
-            if (!has_it) continue;
-            if (iter >= max_iters) status = (id & kIdMask) | kFinalizedMask;
-            ++id;
-        } else {
-            if (!has_res) continue;
-            const V tau = res_kind == 1 ? sqrt(rr) : sqrt(fabs(rho_new));
-            if (tau <= sc[5]) status = kConvergedMask | (id & kIdMask) | kFinalizedMask;
-            ++id;
-        }
-    }
-    ctl[0] = status;
 }
 
 // INIT: r already holds b - A x; computes z, rho, rr (no x/r update) and the baseline.
@@ -181,15 +153,6 @@ __global__ void empty_dot_kernel(V* dot_out, const int32_t* ctl)
 {
     if (ctl && ctl[0] != 0) return;
     *dot_out = V(0);
-}
-
-inline int ew_grid(const b200_ctx* ctx, int64_t n)
-{
-    int64_t g = ceildiv(n, kThreads * 4);
-    const int64_t cap = (int64_t)ctx->num_sms * 4;
-    if (g > cap) g = cap;
-    if (g < 1) g = 1;
-    return (int)g;
 }
 
 }  // namespace fcg
@@ -323,7 +286,7 @@ B200_DEF_FCG(f32, float)
             return B200_OK;                                                                      \
         }                                                                                        \
         b200::csr::DotArgs<VT> dot{work, ctx->counters + 1, dot_out, ctl};                       \
-        return b200::csr::launch_planned<VT, IT, false, true>(                                   \
+        return b200::csr::launch_planned<VT, IT, false, b200::csr::kDotB>(                       \
             ctx, plan, v, nnz, row_ptrs, col_idxs, values, nullptr, b, 1, nullptr, c, 1, dot);   \
     }
 

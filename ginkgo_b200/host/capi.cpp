@@ -83,13 +83,14 @@ std::unique_ptr<LinOp> make_solver(std::shared_ptr<Executor> exec, int kind,
     if (generated_pre && kind == 5) throw NotSupported("make_solver: Ir takes a solver factory");
     if (kind == 0) {
         auto f = solver::Cg<V>::build();
-        f.with_criteria(crit).with_fused(fused != 0).with_check_every(check_every);
+        f.with_criteria(crit).with_fused((fused & 1) != 0).with_check_every(check_every);
         set_pre(f);
         return f.on(exec)->generate(A);
     }
     if (kind == 1) {
         auto f = solver::Bicgstab<V>::build();
-        f.with_criteria(crit);
+        // bit 1 of `fused`: the fused BiCGStab iteration is opt-in, bit 0 keeps meaning Cg's
+        f.with_criteria(crit).with_fused((fused & 2) != 0).with_check_every(check_every);
         set_pre(f);
         return f.on(exec)->generate(A);
     }
@@ -600,7 +601,10 @@ int gkob_csr_kernel_variant(void* csr)
             *iters = (long long)sb->get_num_iterations();                                       \
             *status = sb->get_stop_status(0);                                                   \
             auto cg = dynamic_cast<solver::Cg<V>*>(op);                                         \
-            *used_fused = cg ? (int)cg->used_fused_path() : 0;                                  \
+            auto bicgstab = dynamic_cast<solver::Bicgstab<V>*>(op);                             \
+            *used_fused = cg         ? (int)cg->used_fused_path()                               \
+                          : bicgstab ? (int)bicgstab->used_fused_path()                         \
+                                     : 0;                                                       \
         });                                                                                     \
     }
 GKOB_DEF(double, f64)

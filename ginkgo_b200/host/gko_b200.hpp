@@ -119,6 +119,10 @@ struct viabi;
         static constexpr auto fused_step_p = b200_cg_fused_step_p_##S;                          \
         static constexpr auto fused_step_xr = b200_cg_fused_step_xr_##S;                        \
         static constexpr auto fused_finish = b200_cg_fused_finish_##S;                          \
+        static constexpr auto bicgstab_fused_init = b200_bicgstab_fused_init_##S;               \
+        static constexpr auto bicgstab_fused_step_p = b200_bicgstab_fused_step_p_##S;           \
+        static constexpr auto bicgstab_fused_step_s = b200_bicgstab_fused_step_s_##S;           \
+        static constexpr auto bicgstab_fused_step_xr = b200_bicgstab_fused_step_xr_##S;         \
     };
 GKOB_V(double, f64)
 GKOB_V(float, f32)
@@ -133,6 +137,7 @@ GKOB_V(float, f32)
         static constexpr auto csr_spmv = b200_csr_spmv_##S##_##T;                               \
         static constexpr auto csr_advanced_spmv = b200_csr_advanced_spmv_##S##_##T;             \
         static constexpr auto csr_spmv_dot = b200_csr_spmv_dot_##S##_##T;                       \
+        static constexpr auto csr_spmv_dot2 = b200_csr_spmv_dot2_##S##_##T;                     \
         static constexpr auto csr_extract_diagonal = b200_csr_extract_diagonal_##S##_##T;       \
         static constexpr auto csr_convert_to_ell = b200_csr_convert_to_ell_##S##_##T;           \
         static constexpr auto csr_convert_to_sellp = b200_csr_convert_to_sellp_##S##_##T;       \

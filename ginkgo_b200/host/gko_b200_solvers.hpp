@@ -663,6 +663,50 @@ protected:
         num_iterations_ = iters;
         status_ = stop.to_host();
     }
+    // What the fused device-resident iterations (Cg, Bicgstab) take: a Csr matrix with 16-byte-aligned
+    // arrays, one right-hand side with unit strides and no reducer (rows of a distributed vector take
+    // the loop with its all-reduces), an Identity or scalar-Jacobi preconditioner, and one or two
+    // criteria out of Iteration / (Implicit)ResidualNorm.
+    template <typename I>
+    struct FusedProblem {
+        const matrix::Csr<V, I>* A = nullptr;
+        const V* inv_diag = nullptr;
+        int64 max_iters = -1;
+        int32 res_kind = 0, iter_first = 1, baseline = 0;
+        double factor = 0;
+    };
+    template <typename I>
+    bool fused_problem(const Dense* b, const Dense* x, FusedProblem<I>& f) const
+    {
+        f = FusedProblem<I>{};
+        f.A = dynamic_cast<const matrix::Csr<V, I>*>(system_matrix_.get());
+        if (!f.A || b->get_size().cols != 1 || b->get_stride() != 1 || x->get_stride() != 1) return false;
+        if (b->get_reducer()) return false;
+        if (auto J = dynamic_cast<const preconditioner::Jacobi<V, I>*>(preconditioner_.get())) {
+            if (J->get_max_block_size() != 1) return false;
+            f.inv_diag = J->get_blocks();
+        } else if (!dynamic_cast<const matrix::Identity<V>*>(preconditioner_.get())) {
+            return false;
+        }
+        if (criteria_.empty() || criteria_.size() > 2) return false;
+        for (size_type k = 0; k < criteria_.size(); ++k) {
+            auto& c = criteria_[k];
+            if (c->kind() < 0 || c->kind() > 2) return false;  // e.g. stop::Time: host-side criterion
+            if (c->kind() == 0) {
+                if (f.max_iters >= 0) return false;
+                f.max_iters = (int64)c->max_iters();
+                if (k == 1) f.iter_first = 0;
+            } else {
+                if (f.res_kind) return false;
+                f.res_kind = c->kind();
+                f.factor = c->reduction_factor();
+                f.baseline = c->baseline() == stop::mode::rhs_norm
+                                 ? 0
+                                 : c->baseline() == stop::mode::initial_resnorm ? 1 : 2;
+            }
+        }
+        return !((((std::uintptr_t)f.A->get_const_col_idxs()) | ((std::uintptr_t)f.A->get_const_values())) & 15);
+    }
     std::shared_ptr<const LinOp> system_matrix_;
     std::shared_ptr<const LinOp> preconditioner_;
     std::vector<std::shared_ptr<const stop::CriterionFactory>> criteria_;
@@ -832,43 +876,17 @@ protected:
     template <typename I>
     bool try_fused(const Dense* b, Dense* x) const
     {
-        using Csr = matrix::Csr<V, I>;
-        auto A = dynamic_cast<const Csr*>(this->system_matrix_.get());
-        if (!A || b->get_size().cols != 1 || b->get_stride() != 1 || x->get_stride() != 1) return false;
-        if (b->get_reducer()) return false;  // rows of a distributed vector: the loop with all-reduces
-        const V* inv_diag = nullptr;
-        if (auto J = dynamic_cast<const preconditioner::Jacobi<V, I>*>(this->preconditioner_.get())) {
-            if (J->get_max_block_size() != 1) return false;
-            inv_diag = J->get_blocks();
-        } else if (!dynamic_cast<const matrix::Identity<V>*>(this->preconditioner_.get())) {
-            return false;
-        }
-        int64 max_iters = -1;
-        int32 res_kind = 0, iter_first = 1, baseline = 0;
-        double factor = 0;
-        if (this->criteria_.empty() || this->criteria_.size() > 2) return false;
-        for (size_type k = 0; k < this->criteria_.size(); ++k) {
-            auto& c = this->criteria_[k];
-            if (c->kind() < 0 || c->kind() > 2) return false;  // e.g. stop::Time: host-side criterion
-            if (c->kind() == 0) {
-                if (max_iters >= 0) return false;
-                max_iters = (int64)c->max_iters();
-                if (k == 1) iter_first = 0;
-            } else {
-                if (res_kind) return false;
-                res_kind = c->kind();
-                factor = c->reduction_factor();
-                baseline = c->baseline() == stop::mode::rhs_norm
-                               ? 0
-                               : c->baseline() == stop::mode::initial_resnorm ? 1 : 2;
-            }
-        }
+        typename Base::template FusedProblem<I> f;
+        if (!this->template fused_problem<I>(b, x, f)) return false;
+        const auto A = f.A;
+        const V* inv_diag = f.inv_diag;
+        const int64 max_iters = f.max_iters;
+        const int32 res_kind = f.res_kind, iter_first = f.iter_first, baseline = f.baseline;
+        const double factor = f.factor;
         auto exec = this->exec_;
         auto ctx = exec->ctx();
         const int64 n = this->size_.rows;
         const int64 nnz = A->get_num_stored_elements();
-        if ((((std::uintptr_t)A->get_const_col_idxs()) | ((std::uintptr_t)A->get_const_values())) & 15)
-            return false;
         // workspace (kept across applies: pointers are baked into the iteration graph)
         if (!ws_ || ws_n_ != n) {
             ws_ = Dense::create(exec, dim2{(size_type)(4 * n), 1});
@@ -1641,6 +1659,19 @@ class Bicgstab : public SolverBase<V> {
 
 public:
     struct Factory : SolverFactoryBase<Factory> {
+        bool fused_ = false;
+        int check_every_ = 16;
+        // ginkgo_b200 extension: device-resident fused iteration where applicable (default off)
+        Factory& with_fused(bool f)
+        {
+            fused_ = f;
+            return *this;
+        }
+        Factory& with_check_every(int k)
+        {
+            check_every_ = k;
+            return *this;
+        }
         std::unique_ptr<LinOp> generate(std::shared_ptr<const LinOp> op) const override
         {
             auto exec = this->exec_ ? this->exec_ : op->get_executor();
@@ -1648,16 +1679,21 @@ public:
         }
     };
     static Factory build() { return Factory{}; }
+    bool used_fused_path() const { return used_fused_; }
+    ~Bicgstab() override { b200_graph_destroy(graph_); }
 
 protected:
     Bicgstab(std::shared_ptr<const Executor> exec, const Factory& f, std::shared_ptr<const LinOp> op)
-        : Base(exec, f, op)
+        : Base(exec, f, op), fused_(f.fused_), check_every_(std::max(1, f.check_every_))
     {}
     using Base::apply_impl;
     void apply_impl(const LinOp* lb, LinOp* lx) const override
     {
         auto b = as<Dense>(lb);
         auto x = as<Dense>(lx);
+        if (fused_ && try_fused<int32>(b, x)) return;
+        if (fused_ && try_fused<int64>(b, x)) return;
+        used_fused_ = false;
         auto exec = this->exec_;
         auto ctx = exec->ctx();
         const dim2 sz = b->get_size();
@@ -1723,6 +1759,94 @@ protected:
         }
         this->record(iter, stop_status);
     }
+
+    // Fused device-resident path (csrc/fused_bicgstab.cu): five launches per iteration, a graph of
+    // check_every iterations per read of the control block.
+    template <typename I>
+    bool try_fused(const Dense* b, Dense* x) const
+    {
+        typename Base::template FusedProblem<I> f;
+        if (!this->template fused_problem<I>(b, x, f)) return false;
+        const auto A = f.A;
+        const V* inv_diag = f.inv_diag;
+        auto exec = this->exec_;
+        auto ctx = exec->ctx();
+        const int64 n = this->size_.rows;
+        const int64 nnz = A->get_num_stored_elements();
+        // workspace (kept across applies: pointers are baked into the iteration graph)
+        if (!ws_ || ws_n_ != n) {
+            ws_ = Dense::create(exec, dim2{(size_type)(8 * n), 1});
+            sc_ = array<V>(exec, 16);
+            ctl_ = array<int32>(exec, 8);
+            work_ = array<V>(exec, (size_type)vabi<V>::fused_work_size(ctx));
+            ws_n_ = n;
+            b200_graph_destroy(graph_);
+            graph_ = nullptr;
+        }
+        V* r = ws_->get_values();
+        V *rr = r + n, *p = r + 2 * n, *v = r + 3 * n, *y = r + 4 * n, *s = r + 5 * n, *t = r + 6 * n,
+          *z = r + 7 * n;
+        V* xv = x->get_values();
+        V* sc = sc_.get_data();
+        int32* ctl = ctl_.get_data();
+        // r = b - A x
+        exec->copy(r, b->get_const_values(), n);
+        auto rview = Dense::create_view(exec, dim2{(size_type)n, 1}, r, 1);
+        A->apply(this->neg_one_.get(), x, this->one_.get(), rview.get());
+        if (f.baseline == 0)  // ||b|| into sc[4]
+            GKOB_CALL(vabi<V>::norm2(ctx, n, 1, b->get_const_values(), 1, sc + 4));
+        GKOB_CALL(vabi<V>::bicgstab_fused_init(ctx, n, r, rr, p, v, y, s, t, z, sc, ctl, work_.get_data(),
+                                               f.max_iters, f.res_kind, f.iter_first, f.baseline,
+                                               (V)f.factor));
+        auto spmv_dot2 = [&](const V* in, V* out, const V* w, V* dot, V* dot2) {
+            GKOB_CALL((viabi<V, I>::csr_spmv_dot2(ctx, A->get_plan(), n, n, nnz, A->get_const_row_ptrs(),
+                                                  A->get_const_col_idxs(), A->get_const_values(), in, out,
+                                                  w, dot, dot2, work_.get_data(), ctl)));
+        };
+        auto enqueue_iteration = [&]() {
+            GKOB_CALL(vabi<V>::bicgstab_fused_step_p(ctx, n, p, r, v, y, inv_diag, sc, ctl));
+            spmv_dot2(y, v, rr, sc + 2, nullptr);
+            GKOB_CALL(vabi<V>::bicgstab_fused_step_s(ctx, n, r, v, s, z, inv_diag, sc, ctl, work_.get_data()));
+            spmv_dot2(z, t, s, sc + 8, sc + 2);
+            GKOB_CALL(vabi<V>::bicgstab_fused_step_xr(ctx, n, xv, r, s, t, y, z, rr, sc, ctl, work_.get_data()));
+        };
+        if (!graph_ || graph_x_ != xv || graph_diag_ != inv_diag) {
+            b200_graph_destroy(graph_);
+            graph_ = nullptr;
+            (void)A->get_plan();  // not inside the capture
+            GKOB_CALL(b200_graph_begin_capture(ctx));
+            for (int k = 0; k < check_every_; ++k) enqueue_iteration();
+            GKOB_CALL(b200_graph_end_capture(ctx, &graph_));
+            graph_x_ = xv;
+            graph_diag_ = inv_diag;
+        }
+        // every captured iteration ends with step_xr, so a stop read here has its finalize applied
+        int32 h[8] = {0};
+        exec->copy_to_host(h, ctl_.get_const_data(), 8);
+        while (h[0] == 0) {
+            const int32 before = h[1];
+            GKOB_CALL(b200_graph_launch(ctx, graph_));
+            exec->copy_to_host(h, ctl_.get_const_data(), 8);
+            if (h[0] == 0 && h[1] == before)
+                throw Error("fused BiCGStab: the device iteration made no progress");
+        }
+        this->num_iterations_ = (size_type)h[1];
+        this->status_.assign(1, (uint8)h[0]);
+        used_fused_ = true;
+        return true;
+    }
+
+private:
+    bool fused_;
+    int check_every_;
+    mutable bool used_fused_ = false;
+    mutable std::unique_ptr<Dense> ws_;
+    mutable array<V> sc_, work_;
+    mutable array<int32> ctl_;
+    mutable int64 ws_n_ = -1;
+    mutable b200_graph* graph_ = nullptr;
+    mutable const V* graph_x_ = nullptr;
+    mutable const V* graph_diag_ = nullptr;
 };
 
 // ---------------------------------------------------------------------------------------------

@@ -643,6 +643,68 @@ B200_DECL_SPMV_DOT(f32, float, i32, int32_t)
 B200_DECL_SPMV_DOT(f32, float, i64, int64_t)
 
 /* ---------------------------------------------------------------------------
+ * Fused BiCGStab iteration (ginkgo_b200 extension behind solver::Bicgstab::apply, single GPU;
+ * it regroups the loop body of core/solver/bicgstab.cpp:95-233 into five launches per
+ * iteration with every scalar produced and consumed on the device; d = inv_diag of a
+ * scalar Jacobi preconditioner, NULL for Identity):
+ *   step_p     p = r + (rho/prev_rho*alpha/omega)(p - omega v), p = r if prev_rho*omega == 0;
+ *              y = d.p                                        (bicgstab::step_1 + jacobi apply)
+ *   spmv_dot2  v = A y, beta = rr.v in the SpMV epilogue      (Csr::apply + compute_conj_dot)
+ *   step_s     alpha = rho/beta (0 and s = r if beta == 0); s = r - alpha v; z = d.s; ||s||^2;
+ *              the mid-iteration criterion check on s         (bicgstab::step_2 + norm2 +
+ *                                                              criterion check + jacobi apply)
+ *   spmv_dot2  t = A z, gamma = s.t and beta = t.t            (Csr::apply + 2 compute_conj_dot)
+ *   step_xr    omega = gamma/beta (0 if beta == 0); x += alpha y + omega z; r = s - omega t;
+ *              rho' = rr.r; ||r||^2; rho / prev_rho swapped; iteration count; the top-of-
+ *              iteration criterion check on r                 (bicgstab::step_3 + dot + norm2 +
+ *                                                              criterion check)
+ *   init       r holds b - A x; rr = r; p = v = y = s = t = z = 0; rho = prev_rho = alpha = beta =
+ *              gamma = omega = 1; rho = rr.r, ||r||^2, the baseline and the first check
+ *                                                             (bicgstab::initialize + dot + check)
+ * sc:  VT[16]   0 rho, 1 prev_rho, 2 beta (rr.v, then t.t), 3 ||r||^2, 4 tau0, 5 threshold,
+ *               6 alpha, 7 omega, 8 gamma, 9 ||s||^2
+ * ctl: int32[8] 0 stopping_status byte (0 = running), 1 iterations, 2 max_iters,
+ *               3 res_kind (0 none, 1 ResidualNorm, 2 ImplicitResidualNorm), 4 iter_first,
+ *               5 finalize pending
+ * A stop at the mid check writes the (finalized) status to ctl[0] and sets ctl[5]; step_xr of
+ * the same iteration then only applies bicgstab::finalize, x += alpha y, and clears ctl[5].
+ * With ctl[0] != 0 and ctl[5] == 0 every kernel is a no-op, so graphs of k iterations can be
+ * replayed and the host polls ctl every k iterations.  `work` has b200_cg_fused_work_size
+ * elements; baseline as for the fused CG.
+ *
+ * b200_csr_spmv_dot2: c = A b, *dot_out = w . c and, unless dot2_out is NULL, *dot2_out = c . c
+ * in the epilogue of the SpMV (w: one entry per row; A may be rectangular).  Plan, work, ctl and
+ * alignment rules are those of b200_csr_spmv_dot.
+ * ------------------------------------------------------------------------- */
+#define B200_DECL_FBICGSTAB(V, VT)                                                             \
+    b200_status b200_bicgstab_fused_init_##V(                                                  \
+        b200_ctx* ctx, int64_t n, const VT* r, VT* rr, VT* p, VT* v, VT* y, VT* s, VT* t,      \
+        VT* z, VT* sc, int32_t* ctl, VT* work, int64_t max_iters, int32_t res_kind,            \
+        int32_t iter_first, int32_t baseline, VT reduction_factor);                            \
+    b200_status b200_bicgstab_fused_step_p_##V(b200_ctx* ctx, int64_t n, VT* p, const VT* r,   \
+                                               const VT* v, VT* y, const VT* inv_diag,         \
+                                               const VT* sc, const int32_t* ctl);              \
+    b200_status b200_bicgstab_fused_step_s_##V(b200_ctx* ctx, int64_t n, const VT* r,          \
+                                               const VT* v, VT* s, VT* z, const VT* inv_diag,  \
+                                               VT* sc, int32_t* ctl, VT* work);                \
+    b200_status b200_bicgstab_fused_step_xr_##V(b200_ctx* ctx, int64_t n, VT* x, VT* r,        \
+                                                const VT* s, const VT* t, const VT* y,         \
+                                                const VT* z, const VT* rr, VT* sc,             \
+                                                int32_t* ctl, VT* work);
+#define B200_DECL_SPMV_DOT2(V, VT, I, IT)                                                      \
+    b200_status b200_csr_spmv_dot2_##V##_##I(                                                  \
+        b200_ctx* ctx, const b200_csr_plan* plan, int64_t num_rows, int64_t num_cols,          \
+        int64_t nnz, const IT* row_ptrs, const IT* col_idxs, const VT* values, const VT* b,    \
+        VT* c, const VT* w, VT* dot_out, VT* dot2_out, VT* work, const int32_t* ctl);
+
+B200_DECL_FBICGSTAB(f64, double)
+B200_DECL_FBICGSTAB(f32, float)
+B200_DECL_SPMV_DOT2(f64, double, i32, int32_t)
+B200_DECL_SPMV_DOT2(f64, double, i64, int64_t)
+B200_DECL_SPMV_DOT2(f32, float, i32, int32_t)
+B200_DECL_SPMV_DOT2(f32, float, i64, int64_t)
+
+/* ---------------------------------------------------------------------------
  * Integer-exact helpers either side of the SpMV path (SURVEY.md 8f rank 1):
  * components::convert_ptrs_to_idxs / convert_idxs_to_ptrs
  * (reference/components/format_conversion_kernels.cpp) and csr::extract_diagonal
