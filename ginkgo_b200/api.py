@@ -235,14 +235,16 @@ def _configure_host_lib(h):
     h.gkob_num_cols.restype, h.gkob_num_cols.argtypes = ll, [vp]
     h.gkob_solver_params.restype, h.gkob_solver_params.argtypes = None, [d, d, d]
     h.gkob_solver_guess.restype, h.gkob_solver_guess.argtypes = None, [i]
+    h.gkob_solver_preconditioner.restype, h.gkob_solver_preconditioner.argtypes = None, [vp]
     h.gkob_csr_convert.restype = vp
     h.gkob_csr_convert.argtypes = [vp, ctypes.c_char_p, ll, ll, d, d]
     h.gkob_csr_sort_by_column_index.restype = i
     h.gkob_csr_sort_by_column_index.argtypes = [vp]
     h.gkob_csr_transpose.restype, h.gkob_csr_transpose.argtypes = vp, [vp]
     for s in ("f64", "f32"):
-        f = getattr(h, "gkob_csr_view_%s_i32" % s)
-        f.restype, f.argtypes = vp, [vp, ll, ll, ll, vp, vp, vp]
+        for it in ("i32", "i64"):
+            f = getattr(h, "gkob_csr_view_%s_%s" % (s, it))
+            f.restype, f.argtypes = vp, [vp, ll, ll, ll, vp, vp, vp]
         f = getattr(h, "gkob_dense_view_" + s)
         f.restype, f.argtypes = vp, [vp, ll, ll, ll, vp]
         f = getattr(h, "gkob_solver_create_" + s)
@@ -334,9 +336,9 @@ class _HostObj:
 
 
 def host_csr(exec_, size, values, col_idxs, row_ptrs):
-    """gko_b200::matrix::Csr<V,int32> viewing torch device tensors"""
+    """gko_b200::matrix::Csr<V,int32> (int64 index tensors: Csr<V,int64>) viewing torch device tensors"""
     s = _VT[values.dtype]
-    fn = getattr(_host(), "gkob_csr_view_%s_i32" % s)
+    fn = getattr(_host(), "gkob_csr_view_%s_%s" % (s, "i64" if col_idxs.dtype == torch.int64 else "i32"))
     o = _HostObj(exec_, fn(exec_.h, size[0], size[1], values.numel(), row_ptrs.data_ptr(),
                            col_idxs.data_ptr(), values.data_ptr()), (values, col_idxs, row_ptrs))
     o.vt = s
@@ -507,17 +509,23 @@ class HostSolver:
     1 initial_resnorm / 2 absolute, iter_first = order inside stop::Combined;
     precond_max_bs 0 = none, 1 = scalar Jacobi, k > 1 = block Jacobi (block_ptrs given, or
     detected by find_blocks); for "ir" the preconditioner slot is the inner solver.
-    fused: Cg's device-resident iteration (on where applicable); fused_bicgstab: Bicgstab's, opt-in.
-    used_fused tells after apply whether such a path ran."""
+    fused: Cg's device-resident iteration (on where applicable); fused_bicgstab: Bicgstab's, opt-in;
+    fused_gmres: Gmres's, opt-in (modified Gram-Schmidt, one right-hand side, Identity or any Jacobi,
+    Iteration / ResidualNorm criteria; anything else takes the loop).  check_every: iterations per
+    graph launch on those paths.  preconditioner: a generated one (host_jacobi, e.g. with
+    storage_optimization) used in place of precond_max_bs.  used_fused tells after apply whether such a
+    path ran."""
 
     def __init__(self, exec_, kind, A, precond_max_bs=0, block_ptrs=None, max_iters=None,
                  res_kind=1, baseline=0, reduction=1e-8, iter_first=True, krylov_dim=30, ortho=0,
                  fused=True, check_every=16, relaxation_factor=1.0, foci=(0.0, 1.0), initial_guess="provided",
-                 fused_bicgstab=False):
+                 fused_bicgstab=False, fused_gmres=False, preconditioner=None):
         self.vt = A.vt
         _host().gkob_solver_params(float(relaxation_factor), float(foci[0]), float(foci[1]))
         # "ir" only: solver::initial_guess_mode of with_default_initial_guess
         _host().gkob_solver_guess({"provided": 0, "zero": 1, "rhs": 2}[initial_guess])
+        # a generated preconditioner (host_jacobi) instead of precond_max_bs / block_ptrs
+        _host().gkob_solver_preconditioner(None if preconditioner is None else preconditioner.h)
         bp = None
         nb = 0
         if block_ptrs is not None:
@@ -528,7 +536,8 @@ class HostSolver:
         self.obj = _HostObj(exec_, fn(exec_.h, {"cg": 0, "bicgstab": 1, "gmres": 2, "fcg": 3, "cgs": 4, "ir": 5, "chebyshev": 6, "pipe_cg": 7, "gcr": 8, "minres": 9, "bicg": 10}[kind], A.h,
                                       precond_max_bs, bp, nb, -1 if max_iters is None else max_iters,
                                       res_kind, baseline, reduction, int(iter_first), krylov_dim,
-                                      ortho, int(bool(fused)) | (2 if fused_bicgstab else 0), check_every), (A,))
+                                      ortho, int(bool(fused)) | (2 if fused_bicgstab else 0) |
+                                      (4 if fused_gmres else 0), check_every), (A,))
 
     def apply(self, b, x):
         _hcheck(_host().gkob_apply(self.obj.h, b.h, x.h))

@@ -38,7 +38,7 @@
 namespace b200 {
 namespace fbicgstab {
 
-using namespace fused;  // kThreads, finish_scalars, ew_grid
+using namespace fused;  // kThreads, grid_sums, finish_scalars, ew_grid
 
 template <typename V>
 __global__ void __launch_bounds__(kThreads)
@@ -57,37 +57,6 @@ __global__ void __launch_bounds__(kThreads)
         p[i] = pi;
         y[i] = inv_diag ? pi * inv_diag[i] : pi;
     }
-}
-
-// K sums of one value per thread over the grid: per-CTA partials, a ticket, and the CTA that arrives last
-// adds the partials in a fixed order.  Returns true in that CTA only, whose thread 0 then holds the sums
-// in a[]; the ticket is back at 0.
-template <typename V, int K>
-__device__ __forceinline__ bool grid_sums(V (&a)[K], V* __restrict__ partials, unsigned int* counter, V* red,
-                                          bool* is_last)
-{
-    const int tid = threadIdx.x;
-#pragma unroll
-    for (int k = 0; k < K; ++k) a[k] = block_sum(a[k], red);
-    if (tid == 0) {
-#pragma unroll
-        for (int k = 0; k < K; ++k) partials[K * blockIdx.x + k] = a[k];
-        __threadfence();
-        const unsigned int ticket = atomicAdd(counter, 1u);
-        *is_last = (ticket == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!*is_last) return false;
-    __threadfence();
-#pragma unroll
-    for (int k = 0; k < K; ++k) a[k] = V(0);
-    for (int c = tid; c < (int)gridDim.x; c += kThreads)
-#pragma unroll
-        for (int k = 0; k < K; ++k) a[k] += __ldcg(partials + K * c + k);
-#pragma unroll
-    for (int k = 0; k < K; ++k) a[k] = block_sum(a[k], red);
-    if (tid == 0) *counter = 0u;
-    return true;
 }
 
 // the mid-iteration check on s (core/solver/bicgstab.cpp:170-186), by ONE thread: the criteria of

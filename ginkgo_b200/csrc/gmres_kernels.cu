@@ -8,6 +8,7 @@
 // ((krylov_dim+1)*rows) x cols Dense, basis i = rows [i*rows, (i+1)*rows);
 // hessenberg_iter is the (iter+2) x cols column of the current iteration.
 #include "elementwise.cuh"
+#include "gmres_common.cuh"
 
 namespace b200 {
 namespace gmres {
@@ -55,39 +56,7 @@ __global__ void hessenberg_qr_kernel(int64_t cols, V* gsin, int64_t sins, V* gco
 {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i >= cols || has_stopped(stop[i])) return;
-    final_iter_nums[i]++;
-    V hj = hess[i];
-    for (int64_t j = 0; j < iter; ++j) {
-        const V c = gcos[j * coss + i], s = gsin[j * sins + i];
-        const V hj1 = hess[(j + 1) * hs + i];
-        const V temp = c * hj + s * hj1;
-        const V next = -s * hj + c * hj1;
-        hess[j * hs + i] = temp;
-        hj = next;
-    }
-    // hj == hessenberg(iter), as rotated so far
-    const V this_hess = hj;
-    const V next_hess = hess[(iter + 1) * hs + i];
-    V c, s;
-    if (this_hess == V(0)) {
-        c = V(0);
-        s = V(1);
-    } else {
-        const V scale = fabs(this_hess) + fabs(next_hess);
-        const V a = fabs(this_hess / scale), bq = fabs(next_hess / scale);
-        const V hyp = scale * sqrt(a * a + bq * bq);
-        c = this_hess / hyp;
-        s = next_hess / hyp;
-    }
-    gcos[iter * coss + i] = c;
-    gsin[iter * sins + i] = s;
-    hess[iter * hs + i] = c * this_hess + s * next_hess;
-    hess[(iter + 1) * hs + i] = V(0);
-    const V old = rnc[iter * rncs + i];
-    const V nxt = -s * old;
-    rnc[(iter + 1) * rncs + i] = nxt;
-    rnc[iter * rncs + i] = c * old;
-    residual_norm[i] = fabs(nxt);
+    givens_column(i, gsin, sins, gcos, coss, residual_norm, rnc, rncs, hess, hs, iter, final_iter_nums);
 }
 
 // Back substitution on the transposed-stored Hessenberg:
@@ -146,14 +115,17 @@ struct alignas(sizeof(V) * VW) md_vec {
     V v[VW];
 };
 
-template <typename V, int VW>
+// CTL: the fused GMRES iteration's instance, a no-op once its control word ctl[0] says it stopped.
+template <typename V, int VW, bool CTL = false>
 __global__ void __launch_bounds__(kMdThreads)
     multi_dot_kernel(int64_t rows, int64_t cols, int64_t num_bases, const V* __restrict__ krylov,
                      int64_t ks, const V* __restrict__ w, int64_t wstride, V* __restrict__ partials,
-                     unsigned int* __restrict__ counter, V* __restrict__ hcol, int64_t hs)
+                     unsigned int* __restrict__ counter, V* __restrict__ hcol, int64_t hs,
+                     const int32_t* __restrict__ ctl = nullptr)
 {
     __shared__ V red[32];
     __shared__ bool is_last;
+    if (CTL && ctl[0] != 0) return;
     const int tid = threadIdx.x;
     using vec = md_vec<V, VW>;
     for (int64_t i0 = 0; i0 < num_bases; i0 += kMdMaxBases) {
@@ -257,6 +229,43 @@ b200_status multi_dot(b200_ctx* ctx, int64_t rows, int64_t cols, int64_t num_bas
     return B200_OK;
 }
 
+// h[i] = v_i . w for i < num_bases, one right-hand side, skipped once ctl[0] != 0: the multi-dot of the
+// fused GMRES iteration (CGS / CGS2).  The per-CTA partials live in the caller's workspace at
+// fused_md_offset (the pointer is baked into a graph, ctx->scratch may move), at most
+// kFusedMdCtasPerSm CTAs per SM.
+template <typename V>
+b200_status fused_multi_dot(b200_ctx* ctx, int64_t rows, int64_t num_bases, const V* krylov, const V* w,
+                            V* hcol, const int32_t* ctl, V* work)
+{
+    B200_REQUIRE(ctx && krylov && w && hcol && ctl && work, "null argument");
+    if (num_bases <= 0) return B200_OK;
+    constexpr int kVW = 16 / (int)sizeof(V);
+    const bool vec_ok = rows % kVW == 0 && ((uintptr_t)krylov % 16) == 0 && ((uintptr_t)w % 16) == 0;
+    static thread_local int per_sm[2] = {0, 0};
+    int& occ = per_sm[vec_ok ? 1 : 0];
+    if (occ == 0) {
+        if (vec_ok)
+            B200_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, multi_dot_kernel<V, kVW, true>,
+                                                                          kMdThreads, 0));
+        else
+            B200_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, multi_dot_kernel<V, 1, true>,
+                                                                          kMdThreads, 0));
+        occ = occ < 1 ? 1 : (occ > kFusedMdCtasPerSm ? kFusedMdCtasPerSm : occ);
+    }
+    int grid = (int)ceildiv(rows, (int64_t)kMdThreads * (vec_ok ? kVW : 1) * 2);
+    if (grid > ctx->num_sms * occ) grid = ctx->num_sms * occ;
+    if (grid < 1) grid = 1;
+    V* partials = work + fused_md_offset(ctx);
+    if (vec_ok)
+        multi_dot_kernel<V, kVW, true><<<grid, kMdThreads, 0, ctx->stream>>>(
+            rows, 1, num_bases, krylov, 1, w, 1, partials, ctx->counters + 3, hcol, 1, ctl);
+    else
+        multi_dot_kernel<V, 1, true><<<grid, kMdThreads, 0, ctx->stream>>>(
+            rows, 1, num_bases, krylov, 1, w, 1, partials, ctx->counters + 3, hcol, 1, ctl);
+    B200_LAUNCH_CHECK(ctx);
+    return B200_OK;
+}
+
 }  // namespace gmres
 }  // namespace b200
 
@@ -318,6 +327,13 @@ extern "C" {
     {                                                                                          \
         return b200::gmres::multi_dot<VT>(ctx, rows, cols, num_bases, krylov, ks, next_krylov, \
                                           ns, hcol, hs);                                       \
+    }                                                                                          \
+    b200_status b200_gmres_fused_multi_dot_##V(b200_ctx* ctx, int64_t n, int64_t num_bases,    \
+                                               const VT* krylov, const VT* w, VT* hcol,        \
+                                               const int32_t* ctl, VT* work)                   \
+    {                                                                                          \
+        return b200::gmres::fused_multi_dot<VT>(ctx, n, num_bases, krylov, w, hcol, ctl,       \
+                                                work);                                         \
     }
 
 B200_DEF_GMRES(f64, double)

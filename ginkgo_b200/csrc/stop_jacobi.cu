@@ -104,15 +104,18 @@ namespace jacobi {
 // l / block_offset, so every load of a block column is a single coalesced run for the whole
 // warp.  All MBS columns are fetched before the first multiply (no chain of dependent
 // latencies) and stay in registers for every right-hand side.
-template <typename V, typename I, int MBS, bool ADVANCED, bool ADAPTIVE>
+// CTL: the fused GMRES iteration's instance, a no-op once its control word ctl[0] says it stopped.
+template <typename V, typename I, int MBS, bool ADVANCED, bool ADAPTIVE, bool CTL = false>
 __global__ void __launch_bounds__(256)
     block_apply_kernel(int64_t num_blocks, int64_t block_offset, int64_t group_offset,
                        int32_t group_power, const uint8_t* __restrict__ block_precisions,
                        const I* __restrict__ block_ptrs, const V* __restrict__ blocks,
                        const V* __restrict__ alpha_p,
                        const V* __restrict__ b, int64_t bs_, int64_t num_rhs,
-                       const V* __restrict__ beta_p, V* __restrict__ x, int64_t xs)
+                       const V* __restrict__ beta_p, V* __restrict__ x, int64_t xs,
+                       const int32_t* __restrict__ ctl = nullptr)
 {
+    if (CTL && ctl[0] != 0) return;
     const int lane = threadIdx.x & 31;
     const int64_t group = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     const int group_size = 1 << group_power;
@@ -375,6 +378,44 @@ b200_status block_apply(b200_ctx* ctx, int64_t num_blocks, int32_t max_block_siz
     return B200_OK;
 }
 
+// x = M b for one right-hand side with unit strides, as block_apply's SIMT kernel, skipped once ctl[0] != 0
+// (the preconditioner step of the fused GMRES iteration, replayed in a graph past the stop)
+template <typename V, typename I>
+b200_status fused_block_apply(b200_ctx* ctx, int64_t num_blocks, int32_t max_block_size, int64_t block_offset,
+                              int64_t group_offset, int32_t group_power, const uint8_t* block_precisions,
+                              const I* block_ptrs, const V* blocks, const V* b, V* x, const int32_t* ctl)
+{
+    B200_REQUIRE(ctx != nullptr && ctl != nullptr, "null argument");
+    B200_REQUIRE(max_block_size >= 1 && max_block_size <= 32, "max_block_size must be in [1,32]");
+    B200_REQUIRE(block_offset >= 1 && (block_offset << group_power) <= 32 && group_power >= 0,
+                 "storage scheme does not fit a warp");
+    if (num_blocks <= 0) return B200_OK;
+    const int64_t groups = ceildiv(num_blocks, int64_t(1) << group_power);
+    const unsigned grid = (unsigned)ceildiv(groups * 32, (int64_t)256);
+#define B200_BJC(M)                                                                                 \
+    do {                                                                                            \
+        if (block_precisions)                                                                       \
+            block_apply_kernel<V, I, M, false, true, true><<<grid, 256, 0, ctx->stream>>>(          \
+                num_blocks, block_offset, group_offset, group_power, block_precisions, block_ptrs,  \
+                blocks, nullptr, b, 1, 1, nullptr, x, 1, ctl);                                      \
+        else                                                                                        \
+            block_apply_kernel<V, I, M, false, false, true><<<grid, 256, 0, ctx->stream>>>(         \
+                num_blocks, block_offset, group_offset, group_power, nullptr, block_ptrs, blocks,   \
+                nullptr, b, 1, 1, nullptr, x, 1, ctl);                                              \
+    } while (0)
+    if (block_offset <= 4)
+        B200_BJC(4);
+    else if (block_offset <= 8)
+        B200_BJC(8);
+    else if (block_offset <= 16)
+        B200_BJC(16);
+    else
+        B200_BJC(32);
+#undef B200_BJC
+    B200_LAUNCH_CHECK(ctx);
+    return B200_OK;
+}
+
 }  // namespace jacobi
 }  // namespace b200
 
@@ -481,6 +522,15 @@ B200_DEF_STOP_JACOBI(f32, float)
         return b200::jacobi::block_apply<VT, IT, true>(                                        \
             ctx, num_blocks, max_block_size, block_offset, group_offset, group_power, nullptr, \
             block_pointers, blocks, alpha, b, bs, num_rhs, beta, x, xs);                       \
+    }                                                                                          \
+    b200_status b200_gmres_fused_block_apply_##V##_##I(                                        \
+        b200_ctx* ctx, int64_t num_blocks, int32_t max_block_size, int64_t block_offset,       \
+        int64_t group_offset, int32_t group_power, const uint8_t* block_precisions,            \
+        const IT* block_pointers, const VT* blocks, const VT* b, VT* x, const int32_t* ctl)    \
+    {                                                                                          \
+        return b200::jacobi::fused_block_apply<VT, IT>(                                        \
+            ctx, num_blocks, max_block_size, block_offset, group_offset, group_power,          \
+            block_precisions, block_pointers, blocks, b, x, ctl);                              \
     }
 
 B200_DEF_JACOBI_BLOCK(f64, double, i32, int32_t)

@@ -37,6 +37,8 @@ int guarded(F f)
 // extra parameters of solver kinds 5 (Ir) and 6 (Chebyshev), set by gkob_solver_params
 double g_relaxation = 1.0, g_foci_lo = 0.0, g_foci_hi = 1.0;
 int g_ir_guess = 0;  // kind 5: 0 provided, 1 zero, 2 rhs (gkob_solver_guess)
+// a generated preconditioner for the next gkob_solver_create_* (gkob_solver_preconditioner)
+std::shared_ptr<const LinOp> g_generated_pre;
 
 template <typename V>
 std::unique_ptr<LinOp> make_solver(std::shared_ptr<Executor> exec, int kind,
@@ -147,6 +149,8 @@ std::unique_ptr<LinOp> make_solver(std::shared_ptr<Executor> exec, int kind,
     }
     auto f = solver::Gmres<V>::build();
     f.with_criteria(crit).with_krylov_dim((size_type)krylov_dim);
+    // bit 2 of `fused`: the fused GMRES iteration is opt-in, as BiCGStab's
+    f.with_fused((fused & 4) != 0).with_check_every(check_every);
     f.with_ortho_method(ortho == 0   ? solver::gmres::ortho_method::mgs
                         : ortho == 1 ? solver::gmres::ortho_method::cgs
                                      : solver::gmres::ortho_method::cgs2);
@@ -506,6 +510,9 @@ long long gkob_num_cols(void* op) { return (long long)static_cast<Handle*>(op)->
 // parameters for the next gkob_solver_create_* of kind 5 (Ir: relaxation_factor) or 6
 // (Chebyshev: foci)
 void gkob_solver_guess(int mode) { g_ir_guess = mode; }
+// the next gkob_solver_create_* takes this generated preconditioner (e.g. a gkob_jacobi_create handle)
+// through with_generated_preconditioner instead of precond_max_bs; NULL clears it
+void gkob_solver_preconditioner(void* pre) { g_generated_pre = pre ? static_cast<Handle*>(pre)->op : nullptr; }
 void gkob_solver_params(double relaxation_factor, double foci_lo, double foci_hi)
 {
     g_relaxation = relaxation_factor;
@@ -558,6 +565,21 @@ int gkob_csr_kernel_variant(void* csr)
         }                                                                                       \
         return h;                                                                               \
     }                                                                                           \
+    void* gkob_csr_view_##S##_i64(void* exec, long long n, long long m, long long nnz,         \
+                                  int64* rp, int64* ci, V* va)                                  \
+    {                                                                                           \
+        auto e = static_cast<Handle*>(exec)->exec;                                              \
+        Handle* h = new Handle{e, nullptr};                                                     \
+        if (guarded([&] {                                                                       \
+                h->op = matrix::Csr<V, int64>::create(                                          \
+                    e, dim2{(size_type)n, (size_type)m}, array<V>::view(e, nnz, va),            \
+                    array<int64>::view(e, nnz, ci), array<int64>::view(e, n + 1, rp));          \
+            })) {                                                                               \
+            delete h;                                                                           \
+            return nullptr;                                                                     \
+        }                                                                                       \
+        return h;                                                                               \
+    }                                                                                           \
     void* gkob_dense_view_##S(void* exec, long long rows, long long cols, long long stride,     \
                               V* ptr)                                                           \
     {                                                                                           \
@@ -580,11 +602,13 @@ int gkob_csr_kernel_variant(void* csr)
     {                                                                                           \
         auto e = static_cast<Handle*>(exec)->exec;                                              \
         Handle* h = new Handle{e, nullptr};                                                     \
+        auto gen_pre = std::move(g_generated_pre); /* for this solver only */                   \
+        g_generated_pre = nullptr;                                                              \
         if (guarded([&] {                                                                       \
                 h->op = make_solver<V>(e, kind, static_cast<Handle*>(matrix)->op,               \
                                        precond_max_bs, block_ptrs, nblocks, max_iters,          \
                                        res_kind, baseline, reduction, iter_first, krylov_dim,   \
-                                       ortho, fused, check_every);                              \
+                                       ortho, fused, check_every, gen_pre);                     \
             })) {                                                                               \
             delete h;                                                                           \
             return nullptr;                                                                     \
@@ -602,8 +626,10 @@ int gkob_csr_kernel_variant(void* csr)
             *status = sb->get_stop_status(0);                                                   \
             auto cg = dynamic_cast<solver::Cg<V>*>(op);                                         \
             auto bicgstab = dynamic_cast<solver::Bicgstab<V>*>(op);                             \
+            auto gmres = dynamic_cast<solver::Gmres<V>*>(op);                                   \
             *used_fused = cg         ? (int)cg->used_fused_path()                               \
                           : bicgstab ? (int)bicgstab->used_fused_path()                         \
+                          : gmres    ? (int)gmres->used_fused_path()                            \
                                      : 0;                                                       \
         });                                                                                     \
     }

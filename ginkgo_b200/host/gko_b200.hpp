@@ -123,6 +123,13 @@ struct viabi;
         static constexpr auto bicgstab_fused_step_p = b200_bicgstab_fused_step_p_##S;           \
         static constexpr auto bicgstab_fused_step_s = b200_bicgstab_fused_step_s_##S;           \
         static constexpr auto bicgstab_fused_step_xr = b200_bicgstab_fused_step_xr_##S;         \
+        static constexpr auto gmres_fused_work_size = b200_gmres_fused_work_size_##S;           \
+        static constexpr auto gmres_fused_init = b200_gmres_fused_init_##S;                     \
+        static constexpr auto gmres_fused_scale = b200_gmres_fused_scale_##S;                   \
+        static constexpr auto gmres_fused_mgs_pass = b200_gmres_fused_mgs_pass_##S;             \
+        static constexpr auto gmres_fused_final_pass = b200_gmres_fused_final_pass_##S;         \
+        static constexpr auto gmres_fused_sub_pass = b200_gmres_fused_sub_pass_##S;             \
+        static constexpr auto gmres_fused_multi_dot = b200_gmres_fused_multi_dot_##S;           \
     };
 GKOB_V(double, f64)
 GKOB_V(float, f32)
@@ -170,6 +177,7 @@ GKOB_V(float, f32)
         static constexpr auto jacobi_apply_adaptive = b200_jacobi_apply_adaptive_##S##_##T;     \
         static constexpr auto jacobi_transpose_adaptive =                                       \
             b200_jacobi_transpose_adaptive_##S##_##T;                                           \
+        static constexpr auto gmres_fused_block_apply = b200_gmres_fused_block_apply_##S##_##T; \
     };
 GKOB_VI(double, f64, int32, i32)
 GKOB_VI(double, f64, int64, i64)

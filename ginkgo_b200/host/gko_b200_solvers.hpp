@@ -3,6 +3,7 @@
 #pragma once
 
 #include <chrono>
+#include <functional>
 
 namespace gko_b200 {
 
@@ -663,10 +664,10 @@ protected:
         num_iterations_ = iters;
         status_ = stop.to_host();
     }
-    // What the fused device-resident iterations (Cg, Bicgstab) take: a Csr matrix with 16-byte-aligned
-    // arrays, one right-hand side with unit strides and no reducer (rows of a distributed vector take
-    // the loop with its all-reduces), an Identity or scalar-Jacobi preconditioner, and one or two
-    // criteria out of Iteration / (Implicit)ResidualNorm.
+    // What the fused device-resident iterations (Cg, Bicgstab, Gmres) take: a Csr matrix with
+    // 16-byte-aligned arrays, one right-hand side with unit strides and no reducer (rows of a
+    // distributed vector take the loop with its all-reduces), and one or two criteria out of
+    // Iteration / (Implicit)ResidualNorm.  Which preconditioners each takes is its own rule.
     template <typename I>
     struct FusedProblem {
         const matrix::Csr<V, I>* A = nullptr;
@@ -675,6 +676,18 @@ protected:
         int32 res_kind = 0, iter_first = 1, baseline = 0;
         double factor = 0;
     };
+    // Cg and Bicgstab fold the preconditioner into their element-wise steps: Identity, or scalar
+    // Jacobi with its inverted diagonal in f.inv_diag
+    template <typename I>
+    bool fused_scalar_preconditioner(FusedProblem<I>& f) const
+    {
+        if (auto J = dynamic_cast<const preconditioner::Jacobi<V, I>*>(preconditioner_.get())) {
+            if (J->get_max_block_size() != 1) return false;
+            f.inv_diag = J->get_blocks();
+            return true;
+        }
+        return dynamic_cast<const matrix::Identity<V>*>(preconditioner_.get()) != nullptr;
+    }
     template <typename I>
     bool fused_problem(const Dense* b, const Dense* x, FusedProblem<I>& f) const
     {
@@ -682,12 +695,6 @@ protected:
         f.A = dynamic_cast<const matrix::Csr<V, I>*>(system_matrix_.get());
         if (!f.A || b->get_size().cols != 1 || b->get_stride() != 1 || x->get_stride() != 1) return false;
         if (b->get_reducer()) return false;
-        if (auto J = dynamic_cast<const preconditioner::Jacobi<V, I>*>(preconditioner_.get())) {
-            if (J->get_max_block_size() != 1) return false;
-            f.inv_diag = J->get_blocks();
-        } else if (!dynamic_cast<const matrix::Identity<V>*>(preconditioner_.get())) {
-            return false;
-        }
         if (criteria_.empty() || criteria_.size() > 2) return false;
         for (size_type k = 0; k < criteria_.size(); ++k) {
             auto& c = criteria_[k];
@@ -877,7 +884,8 @@ protected:
     bool try_fused(const Dense* b, Dense* x) const
     {
         typename Base::template FusedProblem<I> f;
-        if (!this->template fused_problem<I>(b, x, f)) return false;
+        if (!this->template fused_problem<I>(b, x, f) || !this->template fused_scalar_preconditioner<I>(f))
+            return false;
         const auto A = f.A;
         const V* inv_diag = f.inv_diag;
         const int64 max_iters = f.max_iters;
@@ -1766,7 +1774,8 @@ protected:
     bool try_fused(const Dense* b, Dense* x) const
     {
         typename Base::template FusedProblem<I> f;
-        if (!this->template fused_problem<I>(b, x, f)) return false;
+        if (!this->template fused_problem<I>(b, x, f) || !this->template fused_scalar_preconditioner<I>(f))
+            return false;
         const auto A = f.A;
         const V* inv_diag = f.inv_diag;
         auto exec = this->exec_;
@@ -1871,6 +1880,20 @@ public:
             ortho_ = m;
             return *this;
         }
+        bool fused_ = false;
+        int check_every_ = 16;  // DESIGN.md 4.5: 8 to 16 are equally fast on an H100, 1 is up to 25 % slower
+        // ginkgo_b200 extension: device-resident fused iteration where applicable (default off)
+        Factory& with_fused(bool f)
+        {
+            fused_ = f;
+            return *this;
+        }
+        // iterations per graph launch (and per read of the control block) on the fused path
+        Factory& with_check_every(int k)
+        {
+            check_every_ = k;
+            return *this;
+        }
         std::unique_ptr<LinOp> generate(std::shared_ptr<const LinOp> op) const override
         {
             auto exec = this->exec_ ? this->exec_ : op->get_executor();
@@ -1878,16 +1901,22 @@ public:
         }
     };
     static Factory build() { return Factory{}; }
+    bool used_fused_path() const { return used_fused_; }
+    ~Gmres() override { drop_graphs(); }
 
 protected:
     Gmres(std::shared_ptr<const Executor> exec, const Factory& f, std::shared_ptr<const LinOp> op)
-        : Base(exec, f, op), krylov_dim_(f.krylov_dim_), ortho_(f.ortho_)
+        : Base(exec, f, op), krylov_dim_(f.krylov_dim_), ortho_(f.ortho_), fused_(f.fused_),
+          check_every_(std::max(1, f.check_every_))
     {}
     using Base::apply_impl;
     void apply_impl(const LinOp* lb, LinOp* lx) const override
     {
         auto b = as<Dense>(lb);
         auto x = as<Dense>(lx);
+        if (fused_ && try_fused<int32>(b, x)) return;
+        if (fused_ && try_fused<int64>(b, x)) return;
+        used_fused_ = false;
         auto exec = this->exec_;
         auto ctx = exec->ctx();
         const dim2 sz = b->get_size();
@@ -2005,9 +2034,206 @@ protected:
 #undef GKOB_CVS
     }
 
+    // Fused device-resident path (csrc/fused_gmres.cu): at Krylov index j, MGS takes j + 3 launches, CGS 4
+    // and CGS2 6 (one more with block Jacobi); the Hessenberg column, the Givens rotations and the stopping
+    // check stay on the device.  One graph per batch of check_every iterations, a batch never crosses a
+    // restart; the host reads the 32-byte control block after each batch.  The initial residual, the
+    // restart and the final update are the loop's kernels, issued by the host.
+    template <typename I>
+    bool try_fused(const Dense* b, Dense* x) const
+    {
+        if (krylov_dim_ == 0) return false;
+        typename Base::template FusedProblem<I> f;
+        // ImplicitResidualNorm: the loop reports NotSupported, and so must this solver
+        if (!this->template fused_problem<I>(b, x, f) || f.res_kind == 2) return false;
+        // any Jacobi (of either index type): scalar (its inverted diagonal), block with given or detected
+        // blocks, adaptive storage
+        const V* inv_diag = nullptr;
+        bool block = false;
+        const void* pre_key[3] = {nullptr, nullptr, nullptr};
+        std::function<void(const V*, V*, const int32*)> block_apply;
+        auto take_jacobi = [&](auto* J) {
+            pre_key[0] = J->get_blocks();
+            pre_key[1] = J->get_block_precisions();
+            if (J->get_max_block_size() == 1) {
+                inv_diag = J->get_blocks();
+                return;
+            }
+            using JI = std::remove_cv_t<std::remove_pointer_t<decltype(J->get_const_block_pointers())>>;
+            pre_key[2] = J->get_const_block_pointers();
+            block = true;
+            block_apply = [J, this](const V* in, V* out, const int32* ctl) {
+                const auto& s = J->get_storage_scheme();
+                GKOB_CALL((viabi<V, JI>::gmres_fused_block_apply(
+                    this->exec_->ctx(), (int64)J->get_num_blocks(), (int32)J->get_max_block_size(), s.block_offset,
+                    s.group_offset, (int32)s.group_power, J->get_block_precisions(), J->get_const_block_pointers(),
+                    J->get_blocks(), in, out, ctl)));
+            };
+        };
+        const LinOp* pre = this->preconditioner_.get();
+        if (auto J = dynamic_cast<const preconditioner::Jacobi<V, int32>*>(pre))
+            take_jacobi(J);
+        else if (auto J = dynamic_cast<const preconditioner::Jacobi<V, int64>*>(pre))
+            take_jacobi(J);
+        else if (!dynamic_cast<const matrix::Identity<V>*>(pre))
+            return false;
+        const auto A = f.A;
+        auto exec = this->exec_;
+        auto ctx = exec->ctx();
+        const int64 n = this->size_.rows, kd = (int64)krylov_dim_;
+        const int64 nnz = A->get_num_stored_elements();
+        // workspace (kept across applies: pointers are baked into the iteration graphs)
+        if (!fkrylov_ || fws_n_ != n) {
+            fkrylov_ = Dense::create(exec, dim2{(size_type)(n * (kd + 1)), 1});
+            fvec_ = Dense::create(exec, dim2{(size_type)(4 * n), 1});  // residual | z | before | after
+            fhess_ = Dense::create(exec, dim2{(size_type)kd, (size_type)(kd + 1)});
+            fsmall_ = array<V>(exec, (size_type)(5 * kd + 11));
+            fwork_ = array<V>(exec, (size_type)vabi<V>::gmres_fused_work_size(ctx, kd));
+            ffin_ = array<std::uint64_t>(exec, 1);
+            fstop_ = array<uint8>(exec, 1);
+            fctl_ = array<int32>(exec, 8);
+            fws_n_ = n;
+            drop_graphs();
+        }
+        // what the graphs bake in besides the workspace: the matrix arrays and its SpMV plan, the
+        // preconditioner's storage
+        const void* key[kGraphKey] = {A->get_const_values(), A->get_const_col_idxs(), A->get_const_row_ptrs(),
+                                      A->get_plan(), pre_key[0], pre_key[1], pre_key[2]};
+        if (!std::equal(key, key + kGraphKey, graph_key_)) {
+            drop_graphs();
+            std::copy(key, key + kGraphKey, graph_key_);
+        }
+        V* K = fkrylov_->get_values();
+        auto col = [&](int c) {
+            return Dense::create_view(exec, dim2{(size_type)n, 1}, fvec_->get_values() + c * n, 1);
+        };
+        auto residual = col(0), z = col(1), before = col(2), after = col(3);
+        V* hess = fhess_->get_values();
+        const int64 hs = fhess_->get_stride();
+        V *sc = fsmall_.get_data(), *gsin = sc + 8, *gcos = gsin + kd, *rnc = gcos + kd, *y = rnc + kd + 1,
+          *rnorm = y + kd, *haux = rnorm + 1;
+        auto rnorm_view = Dense::create_view(exec, dim2{1, 1}, rnorm, 1);
+        std::uint64_t* fin = ffin_.get_data();
+        uint8* stop = fstop_.get_data();
+        int32* ctl = fctl_.get_data();
+        V* work = fwork_.get_data();
+        // the loop's start: fresh Hessenberg, rnc and y; initialize; r = b - A x; ||r||; restart
+        fhess_->fill(V(0));
+        GKOB_CALL(vabi<V>::fill(ctx, 2 * kd + 1, 1, rnc, 1, V(0)));
+        GKOB_CALL(vabi<V>::gmres_initialize(ctx, n, 1, kd, b->get_const_values(), 1, residual->get_values(), 1,
+                                            gsin, 1, gcos, 1, stop));
+        this->system_matrix_->apply(this->neg_one_.get(), x, this->one_.get(), residual.get());
+        residual->compute_norm2(rnorm_view.get());
+        auto restart = [&] {
+            GKOB_CALL(vabi<V>::gmres_restart(ctx, n, 1, residual->get_const_values(), 1, rnorm, rnc, K, 1, fin));
+        };
+        restart();
+        if (f.baseline == 0)  // ||b|| into sc[1]
+            GKOB_CALL(vabi<V>::norm2(ctx, n, 1, b->get_const_values(), 1, sc + 1));
+        GKOB_CALL(vabi<V>::gmres_fused_init(ctx, rnorm, sc, ctl, stop, f.max_iters, f.res_kind, f.iter_first,
+                                            f.baseline, (V)f.factor));
+        auto solve_and_update = [&] {
+            GKOB_CALL(vabi<V>::gmres_solve_krylov(ctx, 1, rnc, 1, hess, hs, y, 1, fin, stop));
+            GKOB_CALL(vabi<V>::gmres_multi_axpy(ctx, n, 1, K, 1, y, 1, before->get_values(), 1, fin, stop));
+            this->preconditioner_->apply(before.get(), after.get());
+            x->add_scaled(this->one_.get(), after.get());
+        };
+        auto enqueue_iteration = [&](int64 j) {
+            V *vj = K + j * n, *w = vj + n, *hcol = hess + j * hs;
+            V* in = vj;
+            if (block) {
+                if (j > 0) GKOB_CALL(vabi<V>::gmres_fused_scale(ctx, n, vj, nullptr, nullptr, sc, ctl, 1));
+                block_apply(vj, z->get_values(), ctl);
+                in = z->get_values();
+            } else if (inv_diag) {
+                GKOB_CALL(vabi<V>::gmres_fused_scale(ctx, n, vj, z->get_values(), inv_diag, sc, ctl, j > 0));
+                in = z->get_values();
+            } else if (j > 0) {
+                GKOB_CALL(vabi<V>::gmres_fused_scale(ctx, n, vj, nullptr, nullptr, sc, ctl, 1));
+            }
+            GKOB_CALL((viabi<V, I>::csr_spmv_dot2(ctx, A->get_plan(), n, n, nnz, A->get_const_row_ptrs(),
+                                                  A->get_const_col_idxs(), A->get_const_values(), in, w, K,
+                                                  hcol, nullptr, work, ctl)));
+            auto final_pass = [&](int64 first, const V* coef, const V* add) {
+                GKOB_CALL(vabi<V>::gmres_fused_final_pass(ctx, n, w, K, first, coef, add, hcol, j, gsin, gcos, rnorm,
+                                                          rnc, fin, stop, sc, ctl, work));
+            };
+            if (ortho_ == gmres::ortho_method::mgs) {
+                for (int64 i = 1; i <= j; ++i)
+                    GKOB_CALL(vabi<V>::gmres_fused_mgs_pass(ctx, n, w, K + (i - 1) * n, K + i * n, hcol, i, ctl,
+                                                            work));
+                final_pass(j, hcol, nullptr);
+                return;
+            }
+            // CGS: h_1..h_j in one pass (h_0 came with the SpMV), one subtract pass over all bases
+            if (j > 0) GKOB_CALL(vabi<V>::gmres_fused_multi_dot(ctx, n, j, K + n, w, hcol + 1, ctl, work));
+            if (ortho_ == gmres::ortho_method::cgs) {
+                final_pass(0, hcol, nullptr);
+                return;
+            }
+            // CGS2: subtract, re-orthogonalise against all bases into haux, subtract again; h += haux
+            GKOB_CALL(vabi<V>::gmres_fused_sub_pass(ctx, n, w, K, hcol, j, ctl));
+            GKOB_CALL(vabi<V>::gmres_fused_multi_dot(ctx, n, j + 1, K, w, haux, ctl, work));
+            final_pass(0, haux, haux);
+        };
+        // batches start at Krylov index 0, c, 2c, ... and end at the restart
+        const int64 ce = std::min<int64>(check_every_, kd);
+        if (graphs_.empty()) {
+            (void)A->get_plan();  // not inside the capture
+            for (int64 j0 = 0; j0 < kd; j0 += ce) {
+                b200_graph* g = nullptr;
+                GKOB_CALL(b200_graph_begin_capture(ctx));
+                for (int64 j = j0; j < std::min(j0 + ce, kd); ++j) enqueue_iteration(j);
+                GKOB_CALL(b200_graph_end_capture(ctx, &g));
+                graphs_.push_back(g);
+            }
+        }
+        int32 h[8] = {0};
+        exec->copy_to_host(h, ctl, 8);
+        int64 j = 0;
+        while (h[0] == 0) {
+            // the loop's restart, only once the check at the top of iteration krylov_dim said "running"
+            if (j == kd) {
+                solve_and_update();
+                residual->copy_from(b);
+                this->system_matrix_->apply(this->neg_one_.get(), x, this->one_.get(), residual.get());
+                residual->compute_norm2(rnorm_view.get());
+                restart();
+                j = 0;
+            }
+            const int32 before_iters = h[1];
+            GKOB_CALL(b200_graph_launch(ctx, graphs_[j / ce]));
+            j = std::min(j + ce, kd);
+            exec->copy_to_host(h, ctl, 8);
+            if (h[0] == 0 && h[1] == before_iters)
+                throw Error("fused GMRES: the device iteration made no progress");
+        }
+        solve_and_update();
+        this->record((size_type)h[1], fstop_);
+        used_fused_ = true;
+        return true;
+    }
+    void drop_graphs() const
+    {
+        for (auto g : graphs_) b200_graph_destroy(g);
+        graphs_.clear();
+    }
+
 private:
     size_type krylov_dim_;
     gmres::ortho_method ortho_;
+    bool fused_;
+    int check_every_;
+    mutable bool used_fused_ = false;
+    mutable std::unique_ptr<Dense> fkrylov_, fvec_, fhess_;
+    mutable array<V> fsmall_, fwork_;
+    mutable array<std::uint64_t> ffin_;
+    mutable array<uint8> fstop_;
+    mutable array<int32> fctl_;
+    mutable int64 fws_n_ = -1;
+    mutable std::vector<b200_graph*> graphs_;
+    static constexpr int kGraphKey = 7;
+    mutable const void* graph_key_[kGraphKey] = {};
 };
 
 }  // namespace solver

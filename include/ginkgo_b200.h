@@ -705,6 +705,79 @@ B200_DECL_SPMV_DOT2(f32, float, i32, int32_t)
 B200_DECL_SPMV_DOT2(f32, float, i64, int64_t)
 
 /* ---------------------------------------------------------------------------
+ * Fused GMRES iteration, modified Gram-Schmidt (ginkgo_b200 extension behind solver::Gmres::apply
+ * with with_fused(true), single GPU; it regroups one iteration of core/solver/gmres.cpp:453-530 at
+ * Krylov index j -- criterion check, preconditioner, SpMV, j+1 dots and sub_scaled, norm2,
+ * inv_scale, hessenberg_qr -- into j + 3 launches (j + 4 with block Jacobi); every Hessenberg
+ * entry, Givens rotation and residual estimate is produced and consumed on the device.  v_i is
+ * Krylov basis i, w = basis j+1, hcol the Hessenberg column of iteration j (h_i = hcol[i]):
+ *   scale        v_j = w / sc[0] if `divide` (the norm of the previous final pass: inv_scale);
+ *                z = inv_diag . v_j unless inv_diag is NULL            (jacobi simple_scalar_apply)
+ *   block_apply  z = M v_j for a block Jacobi M, SIMT kernel of b200_jacobi_simple_apply_* (and
+ *                *_adaptive with block_precisions), one right-hand side, unit strides
+ *   csr_spmv_dot2  w = A z, h_0 = v_0 . w                          (Csr::apply + compute_conj_dot)
+ *   mgs_pass i   w -= h_{i-1} v_{i-1} (skipped for h == 0, as sub_scaled); h_i = v_i . w,
+ *                i = 1..j                                     (sub_scaled + compute_conj_dot)
+ *   final_pass   w -= coef[i] v_i for i = first..j in basis order (each as sub_scaled);
+ *                h_{j+1} = ||w||, also kept in sc[0]; with haux != NULL first hcol[i] += haux[i],
+ *                i <= j (add_scaled); the Givens update of b200_common_gmres_hessenberg_qr on hcol
+ *                with iteration j (gsin, gcos, rnc, rnorm, fin, unit strides); then the criteria on
+ *                tau = rnorm = |rnc[j+1]| for the top of iteration j+1.  MGS: first = j,
+ *                coef = hcol                                  (sub_scaled + norm2 + hessenberg_qr
+ *                                                              + criterion check)
+ * CGS and CGS2 (krylov = v_0, bases at stride n):
+ *   multi_dot    hcol[i] = v_i . w for i < num_bases, one pass (gmres multi_dot); CGS: bases
+ *                1..j into hcol + 1 after the SpMV gave h_0
+ *   final_pass   CGS: first = 0, coef = hcol (the loop's sub_all, then norm2 + hessenberg_qr)
+ *   sub_pass     CGS2: w -= hcol[i] v_i, i = 0..j (sub_all), then multi_dot of bases 0..j into
+ *                haux and final_pass with first = 0, coef = haux, haux = haux
+ *   init         rnorm holds ||b - A x|| and v_0, rnc, fin, gsin, gcos are set by the loop's
+ *                initialize / restart kernels; sets the baseline (sc[1] preset to ||b|| for
+ *                rhs_norm), the threshold and runs the iteration-0 check
+ * sc:  VT[8]    0 ||w|| of the last final pass, 1 tau0, 2 threshold = reduction_factor * tau0
+ * ctl: int32[8] 0 stopping_status byte (0 = running), 1 iterations, 2 max_iters (-1 none),
+ *               3 res_kind (0 none, 1 ResidualNorm), 4 iter_first
+ * Stopping: Iteration and ResidualNorm in the user's order, ids 1 and 2, written WITHOUT the
+ * finalized bit to ctl[0] and to the solver's stop_status byte `stop` (the final solve_krylov /
+ * multi_axpy set it).  With ctl[0] != 0 every kernel above except init is a no-op.  `work` has
+ * b200_gmres_fused_work_size elements; the passes share the ticket of the fused CG step kernels.
+ * ------------------------------------------------------------------------- */
+#define B200_DECL_FGMRES(V, VT)                                                                \
+    int64_t b200_gmres_fused_work_size_##V(const b200_ctx* ctx, int64_t krylov_dim);           \
+    b200_status b200_gmres_fused_init_##V(b200_ctx* ctx, const VT* rnorm, VT* sc, int32_t* ctl, \
+                                          uint8_t* stop, int64_t max_iters, int32_t res_kind,  \
+                                          int32_t iter_first, int32_t baseline,                \
+                                          VT reduction_factor);                                \
+    b200_status b200_gmres_fused_scale_##V(b200_ctx* ctx, int64_t n, VT* v, VT* z,             \
+                                           const VT* inv_diag, const VT* sc,                   \
+                                           const int32_t* ctl, int32_t divide);                \
+    b200_status b200_gmres_fused_mgs_pass_##V(b200_ctx* ctx, int64_t n, VT* w,                 \
+                                              const VT* v_prev, const VT* v_i, VT* hcol,       \
+                                              int64_t i, const int32_t* ctl, VT* work);        \
+    b200_status b200_gmres_fused_sub_pass_##V(b200_ctx* ctx, int64_t n, VT* w,                 \
+                                              const VT* krylov, const VT* coef, int64_t j,     \
+                                              const int32_t* ctl);                             \
+    b200_status b200_gmres_fused_final_pass_##V(                                               \
+        b200_ctx* ctx, int64_t n, VT* w, const VT* krylov, int64_t first, const VT* coef,      \
+        const VT* haux, VT* hcol, int64_t j, VT* gsin, VT* gcos, VT* rnorm, VT* rnc,           \
+        uint64_t* fin, uint8_t* stop, VT* sc, int32_t* ctl, VT* work);                         \
+    b200_status b200_gmres_fused_multi_dot_##V(b200_ctx* ctx, int64_t n, int64_t num_bases,    \
+                                               const VT* krylov, const VT* w, VT* hcol,        \
+                                               const int32_t* ctl, VT* work);
+#define B200_DECL_FGMRES_BLOCK(V, VT, I, IT)                                                   \
+    b200_status b200_gmres_fused_block_apply_##V##_##I(                                        \
+        b200_ctx* ctx, int64_t num_blocks, int32_t max_block_size, int64_t block_offset,       \
+        int64_t group_offset, int32_t group_power, const uint8_t* block_precisions,            \
+        const IT* block_pointers, const VT* blocks, const VT* b, VT* x, const int32_t* ctl);
+
+B200_DECL_FGMRES(f64, double)
+B200_DECL_FGMRES(f32, float)
+B200_DECL_FGMRES_BLOCK(f64, double, i32, int32_t)
+B200_DECL_FGMRES_BLOCK(f64, double, i64, int64_t)
+B200_DECL_FGMRES_BLOCK(f32, float, i32, int32_t)
+B200_DECL_FGMRES_BLOCK(f32, float, i64, int64_t)
+
+/* ---------------------------------------------------------------------------
  * Integer-exact helpers either side of the SpMV path (SURVEY.md 8f rank 1):
  * components::convert_ptrs_to_idxs / convert_idxs_to_ptrs
  * (reference/components/format_conversion_kernels.cpp) and csr::extract_diagonal
