@@ -253,6 +253,8 @@ def _configure_host_lib(h):
         f = getattr(h, "gkob_solver_info_" + s)
         f.restype, f.argtypes = i, [vp, ctypes.POINTER(ll), ctypes.POINTER(ctypes.c_ubyte),
                                     ctypes.POINTER(i)]
+        f = getattr(h, "gkob_solver_statuses_" + s)
+        f.restype, f.argtypes = i, [vp, ctypes.POINTER(ctypes.c_ubyte), ll]
     h.gkob_jacobi_create.restype = vp
     h.gkob_jacobi_create.argtypes = [vp, i, vp, i, vp, ll, i, vp, ll, d]
     h.gkob_jacobi_get.restype, h.gkob_jacobi_get.argtypes = i, [vp, i, vp, vp, vp, vp, vp]
@@ -509,17 +511,20 @@ class HostSolver:
     1 initial_resnorm / 2 absolute, iter_first = order inside stop::Combined;
     precond_max_bs 0 = none, 1 = scalar Jacobi, k > 1 = block Jacobi (block_ptrs given, or
     detected by find_blocks); for "ir" the preconditioner slot is the inner solver.
-    fused: Cg's device-resident iteration (on where applicable); fused_bicgstab: Bicgstab's, opt-in;
+    fused: Cg's device-resident iteration (on where applicable); fused_multi_rhs: Cg's device-resident
+    iteration for 2..32 right-hand sides, opt-in (Csr, b and x without gaps between columns, Identity or
+    scalar Jacobi, Iteration / (Implicit)ResidualNorm; one matrix pass per iteration for all columns,
+    each column stops on its own); fused_bicgstab: Bicgstab's, opt-in;
     fused_gmres: Gmres's, opt-in (modified Gram-Schmidt, one right-hand side, Identity or any Jacobi,
     Iteration / ResidualNorm criteria; anything else takes the loop).  check_every: iterations per
     graph launch on those paths.  preconditioner: a generated one (host_jacobi, e.g. with
     storage_optimization) used in place of precond_max_bs.  used_fused tells after apply whether such a
-    path ran."""
+    path ran; stop_status is column 0's stopping status, stop_statuses every column's."""
 
     def __init__(self, exec_, kind, A, precond_max_bs=0, block_ptrs=None, max_iters=None,
                  res_kind=1, baseline=0, reduction=1e-8, iter_first=True, krylov_dim=30, ortho=0,
                  fused=True, check_every=16, relaxation_factor=1.0, foci=(0.0, 1.0), initial_guess="provided",
-                 fused_bicgstab=False, fused_gmres=False, preconditioner=None):
+                 fused_bicgstab=False, fused_gmres=False, preconditioner=None, fused_multi_rhs=False):
         self.vt = A.vt
         _host().gkob_solver_params(float(relaxation_factor), float(foci[0]), float(foci[1]))
         # "ir" only: solver::initial_guess_mode of with_default_initial_guess
@@ -537,7 +542,8 @@ class HostSolver:
                                       precond_max_bs, bp, nb, -1 if max_iters is None else max_iters,
                                       res_kind, baseline, reduction, int(iter_first), krylov_dim,
                                       ortho, int(bool(fused)) | (2 if fused_bicgstab else 0) |
-                                      (4 if fused_gmres else 0), check_every), (A,))
+                                      (4 if fused_gmres else 0) | (8 if fused_multi_rhs else 0),
+                                      check_every), (A,))
 
     def apply(self, b, x):
         _hcheck(_host().gkob_apply(self.obj.h, b.h, x.h))
@@ -545,6 +551,10 @@ class HostSolver:
         _hcheck(getattr(_host(), "gkob_solver_info_" + self.vt)(self.obj.h, ctypes.byref(it),
                                                                 ctypes.byref(st), ctypes.byref(fu)))
         self.num_iterations, self.stop_status, self.used_fused = it.value, st.value, bool(fu.value)
+        cols = _host().gkob_num_cols(b.h)
+        sts = (ctypes.c_ubyte * max(cols, 1))()
+        _hcheck(getattr(_host(), "gkob_solver_statuses_" + self.vt)(self.obj.h, sts, cols))
+        self.stop_statuses = list(sts[:cols])
         return x
 
 

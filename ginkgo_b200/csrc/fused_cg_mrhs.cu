@@ -1,0 +1,415 @@
+// Fused CG iteration for k = 2..32 right-hand sides of one system, sm_90a: the regrouping of
+// fused_cg.cu with every vector n x k row-major (stride k) and every scalar per column.  One
+// matrix pass per iteration serves all k columns.
+//
+//   step_p    p_j = z_j + (rho_j/prev_rho_j) p_j                     reads 2nk, writes nk
+//   spmv_mdot q = A p for all k columns, pq_j = p_j.q_j in the epilogue  matrix + 2nk (p gathered)
+//   step_xr   alpha_j = rho_j/pq_j; x_j += alpha_j p_j; r_j -= alpha_j q_j; z_j = M^-1 r_j;
+//             rho'_j = r_j.z_j; rr_j = r_j.r_j; per-column check (last CTA)  reads 4nk + n, writes 3nk
+//
+// = matrix + 12 n k + n values per iteration (13 n k in the count of fused_cg.cu, which reads the
+// diagonal once per column), against k (matrix + 13 n) for k one-column solves.  The
+// reference runs the same loop on an n x k Dense and masks every element-wise step by the column's
+// stopping_status (common/unified/solver/cg_kernels.cpp:74,99); so do step_p and step_xr here: a
+// stopped column's x, r and p are not touched again.  The SpMV computes every column (as the
+// reference's Csr::apply does); its q of a stopped column is never read.
+//
+// SpMV layout: that of multi_rhs_rows_kernel (csr_kernels.cuh): P = next power of two >= k lanes
+// per row, lane j gathers column j of the k-wide row of p, every (row, column) sum runs left to
+// right, so q is bit-identical to b200_csr_spmv_* with num_rhs = k.  The grid is bounded and walks
+// the rows grid-stride, so the per-CTA partials (k per CTA, 2k for step_xr) fit a fixed workspace.
+//
+// Sums: per CTA a fixed shuffle tree over the lanes of one column, then the warps in order; the CTA
+// that takes the last ticket adds the CTA partials of each column in a fixed order (one warp per
+// column).  No floating-point atomics: two runs on the same inputs give the same bits.
+//
+// Scalars  sc[6k]:  sc[s*k + j] for column j, s = 0 rho, 1 prev_rho, 2 pq, 3 rr, 4 tau0 (baseline
+//                   norm), 5 threshold = reduction_factor * tau0
+// Status   status[k]: the reference's stopping_status byte of every column (0 = running)
+// Control  ctl[8] (int32): 0 nonzero once EVERY column has stopped, 1 iterations done, 2 max_iters
+//                   (-1 none), 3 res_kind (0 none, 1 ResidualNorm, 2 ImplicitResidualNorm),
+//                   4 iter_first
+// Once ctl[0] != 0 every kernel is a no-op, so a graph of several iterations can be replayed past
+// the stop.
+#include "fused_common.cuh"
+
+namespace b200 {
+namespace fcgm {
+
+using fused::kThreads;  // step kernels
+constexpr int kMaxCols = 32;
+constexpr int kSpmvThreads = 256;
+constexpr int kSpmvCtasPerSm = 8;
+constexpr int kStepCtasPerSm = 4;
+
+inline int lanes_for(int64_t k)
+{
+    int P = 2;
+    while (P < k && P < kMaxCols) P *= 2;
+    return P;
+}
+inline int64_t spmv_cap(const b200_ctx* ctx) { return (int64_t)ctx->num_sms * kSpmvCtasPerSm; }
+inline int64_t step_cap(const b200_ctx* ctx) { return (int64_t)ctx->num_sms * kStepCtasPerSm; }
+
+// rows in flight per CTA sweep = THREADS / P; about 4 sweeps per CTA before the cap is reached
+template <int THREADS>
+inline int rows_grid(int64_t rows, int P, int64_t cap)
+{
+    int64_t g = ceildiv(rows, (int64_t)(THREADS / P) * 4);
+    if (g > cap) g = cap;
+    if (g < 1) g = 1;
+    return (int)g;
+}
+
+// NV sums per column over the CTA: in each warp a fixed shuffle tree over the lanes of one column
+// (lane j, j + P, ...), then the warps in order.  Thread j < P returns column j's sums in a[].
+template <typename V, int P, int NV, int THREADS>
+__device__ __forceinline__ void cta_column_sums(V (&a)[NV], V (&red)[NV][THREADS / 32][P])
+{
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+    for (int off = 16; off >= P; off >>= 1)
+#pragma unroll
+        for (int v = 0; v < NV; ++v) a[v] += __shfl_xor_sync(0xffffffffu, a[v], off);
+    if (lane < P)
+#pragma unroll
+        for (int v = 0; v < NV; ++v) red[v][warp][lane] = a[v];
+    __syncthreads();
+    if (tid < P)
+#pragma unroll
+        for (int v = 0; v < NV; ++v) {
+            V s = V(0);
+            for (int w = 0; w < THREADS / 32; ++w) s += red[v][w][tid];
+            a[v] = s;
+        }
+}
+
+// the grid-wide part: thread j < k publishes its column's NV CTA sums, and the CTA with the last
+// ticket adds the partials of every (sum, column) in CTA order -- one warp per (sum, column), lanes
+// over the CTAs, then a fixed shuffle tree -- into tot[v][j].  Returns true in that CTA only, after a
+// barrier; the ticket is back at 0.
+template <typename V, int NV, int THREADS>
+__device__ __forceinline__ bool grid_column_sums(const V (&a)[NV], int64_t k, V* __restrict__ partials,
+                                                 unsigned int* counter, V (&tot)[NV][kMaxCols], bool* is_last)
+{
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int64_t per_cta = NV * k;
+    if (tid < k) {
+#pragma unroll
+        for (int v = 0; v < NV; ++v) partials[blockIdx.x * per_cta + v * k + tid] = a[v];
+        __threadfence();
+    }
+    __syncthreads();
+    if (tid == 0) {
+        const unsigned int ticket = atomicAdd(counter, 1u);
+        *is_last = (ticket == gridDim.x - 1);
+    }
+    __syncthreads();
+    if (!*is_last) return false;
+    __threadfence();
+    for (int idx = warp; idx < per_cta; idx += THREADS / 32) {
+        V s = V(0);
+        for (int c = lane; c < (int)gridDim.x; c += 32) s += __ldcg(partials + c * per_cta + idx);
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+        if (lane == 0) tot[idx / k][idx % k] = s;
+    }
+    __syncthreads();
+    if (tid == 0) *counter = 0u;
+    return true;
+}
+
+// q = A p for k columns (p, q: stride k), pq_j = sum_i p[i,j] q[i,j] into dots[j]
+template <typename V, typename I, int P>
+__global__ void __launch_bounds__(kSpmvThreads)
+    spmv_mdot_kernel(int64_t num_rows, int64_t k, const I* __restrict__ row_ptrs, const I* __restrict__ col_idxs,
+                     const V* __restrict__ values, const V* __restrict__ b, V* __restrict__ c,
+                     V* __restrict__ dots, V* __restrict__ partials, unsigned int* __restrict__ counter,
+                     const int32_t* __restrict__ ctl)
+{
+    __shared__ V red[1][kSpmvThreads / 32][P];
+    __shared__ V tot[1][kMaxCols];
+    __shared__ bool is_last;
+    if (ctl && ctl[0] != 0) return;
+    constexpr int kRows = kSpmvThreads / P;
+    const int j = threadIdx.x % P;
+    const bool jv = j < k;
+    V a[1] = {V(0)};
+    for (int64_t row = blockIdx.x * (int64_t)kRows + threadIdx.x / P; row < num_rows;
+         row += (int64_t)gridDim.x * kRows) {
+        const int64_t s = row_ptrs[row], e = row_ptrs[row + 1];
+        V acc = V(0);
+        constexpr int kB = 4;
+        for (int64_t t = s; t < e; t += kB) {
+            I cc[kB];
+            V vv[kB], xx[kB];
+#pragma unroll
+            for (int u = 0; u < kB; ++u) {
+                cc[u] = t + u < e ? col_idxs[t + u] : I(0);
+                vv[u] = t + u < e ? values[t + u] : V(0);
+            }
+#pragma unroll
+            for (int u = 0; u < kB; ++u) xx[u] = (t + u < e && jv) ? b[(int64_t)cc[u] * k + j] : V(0);
+#pragma unroll
+            for (int u = 0; u < kB; ++u)
+                if (t + u < e) acc += vv[u] * xx[u];
+        }
+        if (jv) {
+            c[row * k + j] = acc;
+            a[0] += b[row * k + j] * acc;
+        }
+    }
+    cta_column_sums<V, P, 1, kSpmvThreads>(a, red);
+    if (!grid_column_sums<V, 1, kSpmvThreads>(a, k, partials, counter, tot, &is_last)) return;
+    if (threadIdx.x < k) dots[threadIdx.x] = tot[0][threadIdx.x];
+}
+
+template <typename V, int P>
+__global__ void __launch_bounds__(kThreads)
+    step_p_kernel(int64_t n, int64_t k, V* __restrict__ p, const V* __restrict__ z, const V* __restrict__ sc,
+                  const uint8_t* __restrict__ status, const int32_t* __restrict__ ctl)
+{
+    if (ctl[0] != 0) return;
+    constexpr int kRows = kThreads / P;
+    const int j = threadIdx.x % P;
+    if (j >= k || has_stopped(status[j])) return;
+    const V rho = sc[j], prev = sc[k + j];
+    const bool plain = (prev == V(0));
+    const V beta = plain ? V(0) : rho / prev;
+    for (int64_t row = blockIdx.x * (int64_t)kRows + threadIdx.x / P; row < n; row += (int64_t)gridDim.x * kRows) {
+        const int64_t e = row * k + j;
+        const V zi = z[e];
+        p[e] = plain ? zi : zi + beta * p[e];
+    }
+}
+
+// INIT: r already holds b - A x and every column runs; computes z, rho, rr (no x / r update) and
+// each column's baseline
+template <typename V, int P, bool INIT>
+__global__ void __launch_bounds__(kThreads)
+    step_xr_kernel(int64_t n, int64_t k, V* __restrict__ x, V* __restrict__ r, const V* __restrict__ p,
+                   const V* __restrict__ q, V* __restrict__ z, const V* __restrict__ inv_diag, V* __restrict__ sc,
+                   uint8_t* __restrict__ status, int32_t* __restrict__ ctl, V* __restrict__ partials,
+                   unsigned int* __restrict__ counter, int baseline, V factor)
+{
+    __shared__ V red[2][kThreads / 32][P];
+    __shared__ V tot[2][kMaxCols];
+    __shared__ bool is_last;
+    if (!INIT && ctl[0] != 0) return;
+    constexpr int kRows = kThreads / P;
+    const int j = threadIdx.x % P;
+    const bool run = j < k && !has_stopped(status[j]);
+    const V pq = run ? sc[2 * k + j] : V(0);
+    const bool update = !INIT && run && pq != V(0);
+    const V alpha = update ? sc[j] / pq : V(0);
+    V a[2] = {V(0), V(0)};
+    if (run)
+        for (int64_t row = blockIdx.x * (int64_t)kRows + threadIdx.x / P; row < n;
+             row += (int64_t)gridDim.x * kRows) {
+            const int64_t e = row * k + j;
+            V ri = r[e];
+            if (update) {
+                x[e] += alpha * p[e];
+                ri -= alpha * q[e];
+                r[e] = ri;
+            }
+            const V zi = inv_diag ? ri * inv_diag[row] : ri;
+            z[e] = zi;
+            a[0] += ri * zi;
+            a[1] += ri * ri;
+        }
+    cta_column_sums<V, P, 2, kThreads>(a, red);
+    if (!grid_column_sums<V, 2, kThreads>(a, k, partials, counter, tot, &is_last)) return;
+    if (threadIdx.x != 0) return;
+    // the top-of-iteration check of every running column (fused::finish_scalars per column)
+    const int32_t iter = ctl[1] + 1;
+    ctl[1] = iter;
+    bool all_stopped = true;
+    for (int c = 0; c < (int)k; ++c) {
+        uint8_t s = status[c];
+        if (!has_stopped(s)) {
+            const V rho_new = tot[0][c], rr = tot[1][c];
+            if (INIT) {
+                // baseline: 0 rhs_norm (sc[4k + c] preset to ||b_c||), 1 initial_resnorm, 2 absolute
+                if (baseline == 1) sc[4 * k + c] = sqrt(rr);
+                if (baseline == 2) sc[4 * k + c] = V(1);
+                sc[5 * k + c] = factor * sc[4 * k + c];
+            }
+            sc[k + c] = sc[c];
+            sc[c] = rho_new;
+            sc[3 * k + c] = rr;
+            const V threshold = sc[5 * k + c];
+            s = fused::criteria_status(
+                iter, ctl,
+                [&](int32_t res_kind) {
+                    const V tau = res_kind == 1 ? sqrt(rr) : sqrt(fabs(rho_new));
+                    return tau <= threshold;
+                },
+                kFinalizedMask);
+            status[c] = s;
+        }
+        all_stopped = all_stopped && has_stopped(s);
+    }
+    ctl[0] = all_stopped ? 1 : 0;
+}
+
+template <typename V>
+__global__ void init_scalars_kernel(int64_t k, V* sc, uint8_t* status, int32_t* ctl, int32_t max_iters,
+                                    int32_t res_kind, int32_t iter_first)
+{
+    const int j = threadIdx.x;
+    if (j < k) {
+        sc[j] = V(1);  // becomes prev_rho = 1 after the INIT check (reference cg::initialize)
+        sc[k + j] = V(1);
+        sc[2 * k + j] = V(0);
+        sc[3 * k + j] = V(0);
+        status[j] = 0;
+    }
+    if (j == 0) {
+        ctl[0] = 0;
+        ctl[1] = -1;  // the INIT check increments to 0
+        ctl[2] = max_iters;
+        ctl[3] = res_kind;
+        ctl[4] = iter_first;
+    }
+}
+
+// ---- host side of the entry points ----------------------------------------------------------------
+#define B200_FCGM_BY_LANES(P, CALL) \
+    switch (P) {                    \
+    case 2: CALL(2); break;         \
+    case 4: CALL(4); break;         \
+    case 8: CALL(8); break;         \
+    case 16: CALL(16); break;       \
+    default: CALL(32); break;       \
+    }
+
+template <typename V, bool INIT>
+b200_status step_xr(b200_ctx* ctx, int64_t n, int64_t k, V* x, V* r, const V* p, const V* q, V* z,
+                    const V* inv_diag, V* sc, uint8_t* status, int32_t* ctl, V* work, int baseline, V factor)
+{
+    const int P = lanes_for(k);
+    const int grid = rows_grid<kThreads>(n, P, step_cap(ctx));
+    V* partials = work + spmv_cap(ctx) * k;
+#define B200_XR(PP)                                                                                   \
+    step_xr_kernel<V, PP, INIT><<<grid, kThreads, 0, ctx->stream>>>(n, k, x, r, p, q, z, inv_diag, sc, \
+                                                                    status, ctl, partials,            \
+                                                                    ctx->counters + 2, baseline, factor)
+    B200_FCGM_BY_LANES(P, B200_XR)
+#undef B200_XR
+    B200_LAUNCH_CHECK(ctx);
+    return B200_OK;
+}
+
+template <typename V>
+b200_status init(b200_ctx* ctx, int64_t n, int64_t k, const V* r, V* z, V* p, V* q, const V* inv_diag, V* sc,
+                 uint8_t* status, int32_t* ctl, V* work, int64_t max_iters, int32_t res_kind, int32_t iter_first,
+                 int32_t baseline, V factor)
+{
+    B200_REQUIRE(ctx && sc && status && ctl && work, "null argument");
+    B200_REQUIRE(n >= 0 && k >= 2 && k <= kMaxCols, "k must be in [2, 32]");
+    init_scalars_kernel<V><<<1, kMaxCols, 0, ctx->stream>>>(
+        k, sc, status, ctl, (int32_t)(max_iters > 0x7fffffff ? 0x7fffffff : max_iters), res_kind, iter_first);
+    B200_LAUNCH_CHECK(ctx);
+    if (n > 0) {
+        B200_CUDA_CHECK(cudaMemsetAsync(p, 0, sizeof(V) * n * k, ctx->stream));
+        B200_CUDA_CHECK(cudaMemsetAsync(q, 0, sizeof(V) * n * k, ctx->stream));
+    }
+    return step_xr<V, true>(ctx, n, k, nullptr, const_cast<V*>(r), p, q, z, inv_diag, sc, status, ctl, work,
+                            baseline, factor);
+}
+
+template <typename V>
+b200_status step_p(b200_ctx* ctx, int64_t n, int64_t k, V* p, const V* z, const V* sc, const uint8_t* status,
+                   const int32_t* ctl)
+{
+    B200_REQUIRE(ctx && sc && status && ctl, "null argument");
+    B200_REQUIRE(n >= 0 && k >= 2 && k <= kMaxCols, "k must be in [2, 32]");
+    const int P = lanes_for(k);
+    const int grid = rows_grid<kThreads>(n, P, step_cap(ctx));
+#define B200_P(PP) step_p_kernel<V, PP><<<grid, kThreads, 0, ctx->stream>>>(n, k, p, z, sc, status, ctl)
+    B200_FCGM_BY_LANES(P, B200_P)
+#undef B200_P
+    B200_LAUNCH_CHECK(ctx);
+    return B200_OK;
+}
+
+template <typename V, typename I>
+b200_status spmv_mdot(b200_ctx* ctx, int64_t num_rows, int64_t num_cols, int64_t nnz, const I* row_ptrs,
+                      const I* col_idxs, const V* values, const V* b, int64_t k, V* c, V* dots, V* work,
+                      const int32_t* ctl)
+{
+    B200_REQUIRE(ctx && dots && work, "null argument");
+    B200_REQUIRE(num_rows >= 0 && num_cols >= 0 && nnz >= 0, "negative size");
+    B200_REQUIRE(k >= 2 && k <= kMaxCols, "k must be in [2, 32]");
+    B200_REQUIRE(num_rows == 0 || (row_ptrs && c && b), "null pointer");
+    B200_REQUIRE(nnz == 0 || (col_idxs && values), "null pointer");
+    const int P = lanes_for(k);
+    // no rows: one CTA still runs and writes zero dots
+    const int grid = rows_grid<kSpmvThreads>(num_rows, P, spmv_cap(ctx));
+#define B200_MD(PP)                                                                                   \
+    spmv_mdot_kernel<V, I, PP><<<grid, kSpmvThreads, 0, ctx->stream>>>(num_rows, k, row_ptrs, col_idxs, \
+                                                                       values, b, c, dots, work,        \
+                                                                       ctx->counters + 1, ctl)
+    B200_FCGM_BY_LANES(P, B200_MD)
+#undef B200_MD
+    B200_LAUNCH_CHECK(ctx);
+    return B200_OK;
+}
+
+}  // namespace fcgm
+}  // namespace b200
+
+extern "C" {
+
+#define B200_DEF_FCGM(V, VT)                                                                         \
+    /* elements of `work` (value type): SpMV partials (k per CTA), then step_xr's (2k per CTA) */     \
+    int64_t b200_cg_mrhs_work_size_##V(const b200_ctx* ctx, int64_t k)                               \
+    {                                                                                                \
+        return b200::fcgm::spmv_cap(ctx) * k + b200::fcgm::step_cap(ctx) * 2 * k + 64;               \
+    }                                                                                                \
+    b200_status b200_cg_mrhs_init_##V(b200_ctx* ctx, int64_t n, int64_t k, const VT* r, VT* z, VT* p, \
+                                      VT* q, const VT* inv_diag, VT* sc, uint8_t* status, int32_t* ctl, \
+                                      VT* work, int64_t max_iters, int32_t res_kind,                \
+                                      int32_t iter_first, int32_t baseline, VT reduction_factor)    \
+    {                                                                                                \
+        return b200::fcgm::init<VT>(ctx, n, k, r, z, p, q, inv_diag, sc, status, ctl, work, max_iters, \
+                                    res_kind, iter_first, baseline, reduction_factor);               \
+    }                                                                                                \
+    b200_status b200_cg_mrhs_step_p_##V(b200_ctx* ctx, int64_t n, int64_t k, VT* p, const VT* z,     \
+                                        const VT* sc, const uint8_t* status, const int32_t* ctl)     \
+    {                                                                                                \
+        return b200::fcgm::step_p<VT>(ctx, n, k, p, z, sc, status, ctl);                             \
+    }                                                                                                \
+    b200_status b200_cg_mrhs_step_xr_##V(b200_ctx* ctx, int64_t n, int64_t k, VT* x, VT* r,          \
+                                         const VT* p, const VT* q, VT* z, const VT* inv_diag, VT* sc, \
+                                         uint8_t* status, int32_t* ctl, VT* work)                    \
+    {                                                                                                \
+        B200_REQUIRE(ctx && sc && status && ctl && work, "null argument");                           \
+        B200_REQUIRE(n >= 0 && k >= 2 && k <= b200::fcgm::kMaxCols, "k must be in [2, 32]");        \
+        return b200::fcgm::step_xr<VT, false>(ctx, n, k, x, r, p, q, z, inv_diag, sc, status, ctl,   \
+                                              work, 0, VT(0));                                       \
+    }
+
+B200_DEF_FCGM(f64, double)
+B200_DEF_FCGM(f32, float)
+
+/* q = A p for k = 2..32 columns of the row-major p and q (stride k) and dots[j] = p_j . q_j in one */
+/* launch (square A; p is also the dot operand).  `work` provides the per-CTA partials               */
+/* (b200_cg_mrhs_work_size elements); ctl may be NULL.  With num_rows == 0 the dots are 0.          */
+#define B200_DEF_SPMV_MDOT(V, VT, I, IT)                                                             \
+    b200_status b200_csr_spmv_mdot_##V##_##I(b200_ctx* ctx, int64_t num_rows, int64_t num_cols,      \
+                                             int64_t nnz, const IT* row_ptrs, const IT* col_idxs,    \
+                                             const VT* values, const VT* b, int64_t k, VT* c,        \
+                                             VT* dots, VT* work, const int32_t* ctl)                 \
+    {                                                                                                \
+        return b200::fcgm::spmv_mdot<VT, IT>(ctx, num_rows, num_cols, nnz, row_ptrs, col_idxs, values, \
+                                             b, k, c, dots, work, ctl);                              \
+    }
+
+B200_DEF_SPMV_MDOT(f64, double, i32, int32_t)
+B200_DEF_SPMV_MDOT(f64, double, i64, int64_t)
+B200_DEF_SPMV_MDOT(f32, float, i32, int32_t)
+B200_DEF_SPMV_MDOT(f32, float, i64, int64_t)
+
+}  // extern "C"

@@ -86,6 +86,8 @@ std::unique_ptr<LinOp> make_solver(std::shared_ptr<Executor> exec, int kind,
     if (kind == 0) {
         auto f = solver::Cg<V>::build();
         f.with_criteria(crit).with_fused((fused & 1) != 0).with_check_every(check_every);
+        // bit 3 of `fused`: the fused iteration for several right-hand sides is opt-in
+        f.with_fused_multi_rhs((fused & 8) != 0);
         set_pre(f);
         return f.on(exec)->generate(A);
     }
@@ -631,6 +633,15 @@ int gkob_csr_kernel_variant(void* csr)
                           : bicgstab ? (int)bicgstab->used_fused_path()                         \
                           : gmres    ? (int)gmres->used_fused_path()                            \
                                      : 0;                                                       \
+        });                                                                                     \
+    }                                                                                           \
+    /* the stopping status of columns 0..cols-1 after the last apply (0 beyond the solved ones) */ \
+    int gkob_solver_statuses_##S(void* solver, unsigned char* out, long long cols)              \
+    {                                                                                           \
+        return guarded([&] {                                                                    \
+            auto sb = dynamic_cast<solver::SolverBase<V>*>(static_cast<Handle*>(solver)->op.get()); \
+            if (!sb) throw NotSupported("not a solver");                                        \
+            for (long long c = 0; c < cols; ++c) out[c] = sb->get_stop_status((size_type)c);    \
         });                                                                                     \
     }
 GKOB_DEF(double, f64)

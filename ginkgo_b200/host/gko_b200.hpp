@@ -130,6 +130,10 @@ struct viabi;
         static constexpr auto gmres_fused_final_pass = b200_gmres_fused_final_pass_##S;         \
         static constexpr auto gmres_fused_sub_pass = b200_gmres_fused_sub_pass_##S;             \
         static constexpr auto gmres_fused_multi_dot = b200_gmres_fused_multi_dot_##S;           \
+        static constexpr auto cg_mrhs_work_size = b200_cg_mrhs_work_size_##S;                   \
+        static constexpr auto cg_mrhs_init = b200_cg_mrhs_init_##S;                             \
+        static constexpr auto cg_mrhs_step_p = b200_cg_mrhs_step_p_##S;                         \
+        static constexpr auto cg_mrhs_step_xr = b200_cg_mrhs_step_xr_##S;                       \
     };
 GKOB_V(double, f64)
 GKOB_V(float, f32)
@@ -145,6 +149,7 @@ GKOB_V(float, f32)
         static constexpr auto csr_advanced_spmv = b200_csr_advanced_spmv_##S##_##T;             \
         static constexpr auto csr_spmv_dot = b200_csr_spmv_dot_##S##_##T;                       \
         static constexpr auto csr_spmv_dot2 = b200_csr_spmv_dot2_##S##_##T;                     \
+        static constexpr auto csr_spmv_mdot = b200_csr_spmv_mdot_##S##_##T;                     \
         static constexpr auto csr_extract_diagonal = b200_csr_extract_diagonal_##S##_##T;       \
         static constexpr auto csr_convert_to_ell = b200_csr_convert_to_ell_##S##_##T;           \
         static constexpr auto csr_convert_to_sellp = b200_csr_convert_to_sellp_##S##_##T;       \

@@ -665,9 +665,10 @@ protected:
         status_ = stop.to_host();
     }
     // What the fused device-resident iterations (Cg, Bicgstab, Gmres) take: a Csr matrix with
-    // 16-byte-aligned arrays, one right-hand side with unit strides and no reducer (rows of a
-    // distributed vector take the loop with its all-reduces), and one or two criteria out of
-    // Iteration / (Implicit)ResidualNorm.  Which preconditioners each takes is its own rule.
+    // 16-byte-aligned arrays, 1..max_cols right-hand sides stored without gaps (stride == columns)
+    // and no reducer (rows of a distributed vector take the loop with its all-reduces), and one or
+    // two criteria out of Iteration / (Implicit)ResidualNorm.  Which preconditioners each takes is
+    // its own rule; every caller but Cg's several-column path accepts one column.
     template <typename I>
     struct FusedProblem {
         const matrix::Csr<V, I>* A = nullptr;
@@ -689,11 +690,13 @@ protected:
         return dynamic_cast<const matrix::Identity<V>*>(preconditioner_.get()) != nullptr;
     }
     template <typename I>
-    bool fused_problem(const Dense* b, const Dense* x, FusedProblem<I>& f) const
+    bool fused_problem(const Dense* b, const Dense* x, FusedProblem<I>& f, size_type max_cols = 1) const
     {
         f = FusedProblem<I>{};
         f.A = dynamic_cast<const matrix::Csr<V, I>*>(system_matrix_.get());
-        if (!f.A || b->get_size().cols != 1 || b->get_stride() != 1 || x->get_stride() != 1) return false;
+        const size_type cols = b->get_size().cols;
+        if (!f.A || cols < 1 || cols > max_cols || b->get_stride() != cols || x->get_stride() != cols)
+            return false;
         if (b->get_reducer()) return false;
         if (criteria_.empty() || criteria_.size() > 2) return false;
         for (size_type k = 0; k < criteria_.size(); ++k) {
@@ -793,11 +796,19 @@ class Cg : public SolverBase<V> {
 public:
     struct Factory : SolverFactoryBase<Factory> {
         bool fused_ = true;
+        bool fused_multi_rhs_ = false;
         int check_every_ = 16;
         // ginkgo_b200 extension: device-resident fused iteration (default on where applicable)
         Factory& with_fused(bool f)
         {
             fused_ = f;
+            return *this;
+        }
+        // ginkgo_b200 extension: the device-resident iteration for 2..32 right-hand sides, one
+        // matrix pass per iteration for all columns (opt-in)
+        Factory& with_fused_multi_rhs(bool f)
+        {
+            fused_multi_rhs_ = f;
             return *this;
         }
         Factory& with_check_every(int k)
@@ -813,11 +824,16 @@ public:
     };
     static Factory build() { return Factory{}; }
     bool used_fused_path() const { return used_fused_; }
-    ~Cg() override { b200_graph_destroy(graph_); }
+    ~Cg() override
+    {
+        b200_graph_destroy(graph_);
+        b200_graph_destroy(mrhs_.graph);
+    }
 
 protected:
     Cg(std::shared_ptr<const Executor> exec, const Factory& f, std::shared_ptr<const LinOp> op)
-        : Base(exec, f, op), fused_(f.fused_), check_every_(std::max(1, f.check_every_))
+        : Base(exec, f, op), fused_(f.fused_), fused_multi_rhs_(f.fused_multi_rhs_),
+          check_every_(std::max(1, f.check_every_))
     {}
     using Base::apply_impl;
 
@@ -827,6 +843,8 @@ protected:
         auto dx = as<Dense>(x);
         if (fused_ && try_fused<int32>(db, dx)) return;
         if (fused_ && try_fused<int64>(db, dx)) return;
+        if (fused_multi_rhs_ && try_fused_multi_rhs<int32>(db, dx)) return;
+        if (fused_multi_rhs_ && try_fused_multi_rhs<int64>(db, dx)) return;
         used_fused_ = false;
         apply_dense_impl(db, dx);
     }
@@ -957,8 +975,91 @@ protected:
         return true;
     }
 
+    // Fused device-resident path for k = 2..32 right-hand sides (csrc/fused_cg_mrhs.cu): the same
+    // admission as try_fused but with b and x of k columns stored without gaps.  Every column stops
+    // on its own; the device keeps a stopped column's x, r and p as the loop's masked steps leave
+    // them, and the host reads all k statuses at the end.
+    template <typename I>
+    bool try_fused_multi_rhs(const Dense* b, Dense* x) const
+    {
+        typename Base::template FusedProblem<I> f;
+        if (b->get_size().cols < 2 || !this->template fused_problem<I>(b, x, f, 32) ||
+            !this->template fused_scalar_preconditioner<I>(f))
+            return false;
+        const auto A = f.A;
+        auto exec = this->exec_;
+        auto ctx = exec->ctx();
+        const int64 n = this->size_.rows;
+        const int64 k = (int64)b->get_size().cols;
+        const int64 nnz = A->get_num_stored_elements();
+        auto& m = mrhs_;
+        // workspace r, z, p, q (n x k each), per-column scalars, statuses, control block, partials;
+        // kept across applies
+        if (!m.ws || m.n != n || m.k != k) {
+            m.ws = Dense::create(exec, dim2{(size_type)(4 * n * k), 1});
+            m.sc = array<V>(exec, (size_type)(6 * k));
+            m.status = array<uint8>(exec, (size_type)k);
+            m.ctl = array<int32>(exec, 8);
+            m.work = array<V>(exec, (size_type)vabi<V>::cg_mrhs_work_size(ctx, k));
+            m.n = n;
+            m.k = k;
+            b200_graph_destroy(m.graph);  // it holds the pointers just freed
+            m.graph = nullptr;
+        }
+        V* r = m.ws->get_values();
+        V* z = r + n * k;
+        V* p = z + n * k;
+        V* q = p + n * k;
+        V* xv = x->get_values();
+        V* sc = m.sc.get_data();
+        // r = b - A x
+        exec->copy(r, b->get_const_values(), n * k);
+        auto rview = Dense::create_view(exec, dim2{(size_type)n, (size_type)k}, r, (size_type)k);
+        A->apply(this->neg_one_.get(), x, this->one_.get(), rview.get());
+        if (f.baseline == 0)  // ||b_j|| into sc[4k + j]
+            GKOB_CALL(vabi<V>::norm2(ctx, n, k, b->get_const_values(), k, sc + 4 * k));
+        GKOB_CALL(vabi<V>::cg_mrhs_init(ctx, n, k, r, z, p, q, f.inv_diag, sc, m.status.get_data(),
+                                        m.ctl.get_data(), m.work.get_data(), f.max_iters, f.res_kind,
+                                        f.iter_first, f.baseline, (V)f.factor));
+        // the graph bakes in every pointer and size below: re-capture when one changes
+        const MultiRhsKey key{k, r, xv, f.inv_diag, A->get_const_row_ptrs(), A->get_const_col_idxs(),
+                              A->get_const_values(), nnz};
+        if (!m.graph || !(m.key == key)) {
+            b200_graph_destroy(m.graph);
+            m.graph = nullptr;
+            GKOB_CALL(b200_graph_begin_capture(ctx));
+            for (int it = 0; it < check_every_; ++it) {
+                GKOB_CALL(vabi<V>::cg_mrhs_step_p(ctx, n, k, p, z, sc, m.status.get_const_data(),
+                                                  m.ctl.get_const_data()));
+                GKOB_CALL((viabi<V, I>::csr_spmv_mdot(ctx, n, n, nnz, A->get_const_row_ptrs(),
+                                                      A->get_const_col_idxs(), A->get_const_values(), p, k,
+                                                      q, sc + 2 * k, m.work.get_data(),
+                                                      m.ctl.get_const_data())));
+                GKOB_CALL(vabi<V>::cg_mrhs_step_xr(ctx, n, k, xv, r, p, q, z, f.inv_diag, sc,
+                                                   m.status.get_data(), m.ctl.get_data(),
+                                                   m.work.get_data()));
+            }
+            GKOB_CALL(b200_graph_end_capture(ctx, &m.graph));
+            m.key = key;
+        }
+        int32 h[8] = {0};
+        exec->copy_to_host(h, m.ctl.get_const_data(), 8);
+        while (h[0] == 0) {
+            const int32 before = h[1];
+            GKOB_CALL(b200_graph_launch(ctx, m.graph));
+            exec->copy_to_host(h, m.ctl.get_const_data(), 8);
+            if (h[0] == 0 && h[1] == before)
+                throw Error("fused CG (several right-hand sides): the device iteration made no progress");
+        }
+        this->num_iterations_ = (size_type)h[1];
+        this->status_ = m.status.to_host();
+        used_fused_ = true;
+        return true;
+    }
+
 private:
     bool fused_;
+    bool fused_multi_rhs_;
     int check_every_;
     mutable bool used_fused_ = false;
     mutable std::unique_ptr<Dense> ws_;
@@ -968,6 +1069,32 @@ private:
     mutable b200_graph* graph_ = nullptr;
     mutable const V* graph_x_ = nullptr;
     mutable const V* graph_diag_ = nullptr;
+    // what the several-column graph bakes in (the index arrays as untyped pointers: int32 or int64)
+    struct MultiRhsKey {
+        int64 k = 0;
+        const V* ws = nullptr;
+        const V* x = nullptr;
+        const V* inv_diag = nullptr;
+        const void* row_ptrs = nullptr;
+        const void* col_idxs = nullptr;
+        const V* values = nullptr;
+        int64 nnz = -1;
+        bool operator==(const MultiRhsKey& o) const
+        {
+            return k == o.k && ws == o.ws && x == o.x && inv_diag == o.inv_diag && row_ptrs == o.row_ptrs &&
+                   col_idxs == o.col_idxs && values == o.values && nnz == o.nnz;
+        }
+    };
+    struct MultiRhsState {
+        std::unique_ptr<Dense> ws;
+        array<V> sc, work;
+        array<uint8> status;
+        array<int32> ctl;
+        int64 n = -1, k = 0;
+        b200_graph* graph = nullptr;
+        MultiRhsKey key;
+    };
+    mutable MultiRhsState mrhs_;
 };
 
 // ---------------------------------------------------------------------------------------------

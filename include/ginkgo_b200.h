@@ -705,6 +705,61 @@ B200_DECL_SPMV_DOT2(f32, float, i32, int32_t)
 B200_DECL_SPMV_DOT2(f32, float, i64, int64_t)
 
 /* ---------------------------------------------------------------------------
+ * Fused CG iteration for k = 2..32 right-hand sides (ginkgo_b200 extension behind solver::Cg::apply
+ * with with_fused_multi_rhs(true), single GPU).  The regrouping of the fused CG above with every
+ * vector n x k row-major (stride k) and every scalar per column; one matrix pass per iteration
+ * serves all columns.  The element-wise steps of a stopped column are skipped, as the reference's
+ * cg::step_1 / step_2 skip them by the column's stopping_status
+ * (common/unified/solver/cg_kernels.cpp:74,99):
+ *   step_p     p_j = z_j + (rho_j/prev_rho_j) p_j; p_j = z_j if prev_rho_j == 0   (cg::step_1)
+ *   spmv_mdot  q = A p for all columns, pq_j = p_j . q_j in the SpMV epilogue
+ *                                                (Csr::apply with k columns + compute_conj_dot)
+ *   step_xr    alpha_j = rho_j/pq_j (no update if pq_j == 0); x_j += alpha_j p_j;
+ *              r_j -= alpha_j q_j; z_j = M^-1 r_j (scalar Jacobi or identity); rho'_j = r_j . z_j;
+ *              rr_j = r_j . r_j; the Iteration / (Implicit)ResidualNorm check of every running
+ *              column                            (cg::step_2 + jacobi apply + dot + norm2 + check)
+ *   init       r holds b - A x; p = q = 0; rho = prev_rho = 1; all columns running; z, rho, rr,
+ *              each column's baseline and the first check        (cg::initialize + dot + check)
+ * sc:     VT[6k]    sc[s*k + j]: s = 0 rho, 1 prev_rho, 2 pq, 3 rr, 4 tau0, 5 threshold
+ * status: uint8[k]  stopping_status byte of every column (0 = running)
+ * ctl:    int32[8]  0 nonzero once every column has stopped, 1 iterations, 2 max_iters,
+ *                   3 res_kind (0 none, 1 ResidualNorm, 2 ImplicitResidualNorm), 4 iter_first
+ * Once ctl[0] != 0 every kernel is a no-op, so graphs of several iterations can be replayed and the
+ * host polls ctl after each.  `work` has b200_cg_mrhs_work_size(k) elements.  baseline: 0 rhs_norm
+ * (caller stores ||b_j|| in sc[4k + j] first), 1 initial_resnorm, 2 absolute.
+ *
+ * b200_csr_spmv_mdot: c = A b for the k columns of the row-major b and c (stride k; square A, b
+ * also the dot operand) and dots[j] = b_j . c_j.  c is bit-identical to b200_csr_spmv with
+ * num_rhs = k; the dots are summed in a fixed order.  ctl may be NULL; with num_rows == 0 the dots
+ * are 0.  No plan and no alignment are required.
+ * ------------------------------------------------------------------------- */
+#define B200_DECL_FCGM(V, VT)                                                                  \
+    int64_t b200_cg_mrhs_work_size_##V(const b200_ctx* ctx, int64_t k);                        \
+    b200_status b200_cg_mrhs_init_##V(b200_ctx* ctx, int64_t n, int64_t k, const VT* r, VT* z, \
+                                      VT* p, VT* q, const VT* inv_diag, VT* sc,                \
+                                      uint8_t* status, int32_t* ctl, VT* work,                 \
+                                      int64_t max_iters, int32_t res_kind, int32_t iter_first, \
+                                      int32_t baseline, VT reduction_factor);                  \
+    b200_status b200_cg_mrhs_step_p_##V(b200_ctx* ctx, int64_t n, int64_t k, VT* p,            \
+                                        const VT* z, const VT* sc, const uint8_t* status,      \
+                                        const int32_t* ctl);                                   \
+    b200_status b200_cg_mrhs_step_xr_##V(b200_ctx* ctx, int64_t n, int64_t k, VT* x, VT* r,    \
+                                         const VT* p, const VT* q, VT* z, const VT* inv_diag,  \
+                                         VT* sc, uint8_t* status, int32_t* ctl, VT* work);
+#define B200_DECL_SPMV_MDOT(V, VT, I, IT)                                                      \
+    b200_status b200_csr_spmv_mdot_##V##_##I(                                                  \
+        b200_ctx* ctx, int64_t num_rows, int64_t num_cols, int64_t nnz, const IT* row_ptrs,    \
+        const IT* col_idxs, const VT* values, const VT* b, int64_t k, VT* c, VT* dots,         \
+        VT* work, const int32_t* ctl);
+
+B200_DECL_FCGM(f64, double)
+B200_DECL_FCGM(f32, float)
+B200_DECL_SPMV_MDOT(f64, double, i32, int32_t)
+B200_DECL_SPMV_MDOT(f64, double, i64, int64_t)
+B200_DECL_SPMV_MDOT(f32, float, i32, int32_t)
+B200_DECL_SPMV_MDOT(f32, float, i64, int64_t)
+
+/* ---------------------------------------------------------------------------
  * Fused GMRES iteration, modified Gram-Schmidt (ginkgo_b200 extension behind solver::Gmres::apply
  * with with_fused(true), single GPU; it regroups one iteration of core/solver/gmres.cpp:453-530 at
  * Krylov index j -- criterion check, preconditioner, SpMV, j+1 dots and sub_scaled, norm2,
