@@ -14,14 +14,9 @@
 // stopped column's x, r and p are not touched again.  The SpMV computes every column (as the
 // reference's Csr::apply does); its q of a stopped column is never read.
 //
-// SpMV layout: that of multi_rhs_rows_kernel (csr_kernels.cuh): P = next power of two >= k lanes
-// per row, lane j gathers column j of the k-wide row of p, every (row, column) sum runs left to
-// right, so q is bit-identical to b200_csr_spmv_* with num_rhs = k.  The grid is bounded and walks
-// the rows grid-stride, so the per-CTA partials (k per CTA, 2k for step_xr) fit a fixed workspace.
-//
-// Sums: per CTA a fixed shuffle tree over the lanes of one column, then the warps in order; the CTA
-// that takes the last ticket adds the CTA partials of each column in a fixed order (one warp per
-// column).  No floating-point atomics: two runs on the same inputs give the same bits.
+// Row / lane layout, bounded grids, per-column sums and the SpMV (its DotB epilogue) are those of
+// fused_mrhs.cuh: q is bit-identical to b200_csr_spmv_* with num_rhs = k, and the per-CTA partials
+// (k per CTA, 2k for step_xr) fit a fixed workspace.
 //
 // Scalars  sc[6k]:  sc[s*k + j] for column j, s = 0 rho, 1 prev_rho, 2 pq, 3 rr, 4 tau0 (baseline
 //                   norm), 5 threshold = reduction_factor * tau0
@@ -31,138 +26,13 @@
 //                   4 iter_first
 // Once ctl[0] != 0 every kernel is a no-op, so a graph of several iterations can be replayed past
 // the stop.
-#include "fused_common.cuh"
+#include "fused_mrhs.cuh"
 
 namespace b200 {
 namespace fcgm {
 
 using fused::kThreads;  // step kernels
-constexpr int kMaxCols = 32;
-constexpr int kSpmvThreads = 256;
-constexpr int kSpmvCtasPerSm = 8;
-constexpr int kStepCtasPerSm = 4;
-
-inline int lanes_for(int64_t k)
-{
-    int P = 2;
-    while (P < k && P < kMaxCols) P *= 2;
-    return P;
-}
-inline int64_t spmv_cap(const b200_ctx* ctx) { return (int64_t)ctx->num_sms * kSpmvCtasPerSm; }
-inline int64_t step_cap(const b200_ctx* ctx) { return (int64_t)ctx->num_sms * kStepCtasPerSm; }
-
-// rows in flight per CTA sweep = THREADS / P; about 4 sweeps per CTA before the cap is reached
-template <int THREADS>
-inline int rows_grid(int64_t rows, int P, int64_t cap)
-{
-    int64_t g = ceildiv(rows, (int64_t)(THREADS / P) * 4);
-    if (g > cap) g = cap;
-    if (g < 1) g = 1;
-    return (int)g;
-}
-
-// NV sums per column over the CTA: in each warp a fixed shuffle tree over the lanes of one column
-// (lane j, j + P, ...), then the warps in order.  Thread j < P returns column j's sums in a[].
-template <typename V, int P, int NV, int THREADS>
-__device__ __forceinline__ void cta_column_sums(V (&a)[NV], V (&red)[NV][THREADS / 32][P])
-{
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-#pragma unroll
-    for (int off = 16; off >= P; off >>= 1)
-#pragma unroll
-        for (int v = 0; v < NV; ++v) a[v] += __shfl_xor_sync(0xffffffffu, a[v], off);
-    if (lane < P)
-#pragma unroll
-        for (int v = 0; v < NV; ++v) red[v][warp][lane] = a[v];
-    __syncthreads();
-    if (tid < P)
-#pragma unroll
-        for (int v = 0; v < NV; ++v) {
-            V s = V(0);
-            for (int w = 0; w < THREADS / 32; ++w) s += red[v][w][tid];
-            a[v] = s;
-        }
-}
-
-// the grid-wide part: thread j < k publishes its column's NV CTA sums, and the CTA with the last
-// ticket adds the partials of every (sum, column) in CTA order -- one warp per (sum, column), lanes
-// over the CTAs, then a fixed shuffle tree -- into tot[v][j].  Returns true in that CTA only, after a
-// barrier; the ticket is back at 0.
-template <typename V, int NV, int THREADS>
-__device__ __forceinline__ bool grid_column_sums(const V (&a)[NV], int64_t k, V* __restrict__ partials,
-                                                 unsigned int* counter, V (&tot)[NV][kMaxCols], bool* is_last)
-{
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int64_t per_cta = NV * k;
-    if (tid < k) {
-#pragma unroll
-        for (int v = 0; v < NV; ++v) partials[blockIdx.x * per_cta + v * k + tid] = a[v];
-        __threadfence();
-    }
-    __syncthreads();
-    if (tid == 0) {
-        const unsigned int ticket = atomicAdd(counter, 1u);
-        *is_last = (ticket == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!*is_last) return false;
-    __threadfence();
-    for (int idx = warp; idx < per_cta; idx += THREADS / 32) {
-        V s = V(0);
-        for (int c = lane; c < (int)gridDim.x; c += 32) s += __ldcg(partials + c * per_cta + idx);
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-        if (lane == 0) tot[idx / k][idx % k] = s;
-    }
-    __syncthreads();
-    if (tid == 0) *counter = 0u;
-    return true;
-}
-
-// q = A p for k columns (p, q: stride k), pq_j = sum_i p[i,j] q[i,j] into dots[j]
-template <typename V, typename I, int P>
-__global__ void __launch_bounds__(kSpmvThreads)
-    spmv_mdot_kernel(int64_t num_rows, int64_t k, const I* __restrict__ row_ptrs, const I* __restrict__ col_idxs,
-                     const V* __restrict__ values, const V* __restrict__ b, V* __restrict__ c,
-                     V* __restrict__ dots, V* __restrict__ partials, unsigned int* __restrict__ counter,
-                     const int32_t* __restrict__ ctl)
-{
-    __shared__ V red[1][kSpmvThreads / 32][P];
-    __shared__ V tot[1][kMaxCols];
-    __shared__ bool is_last;
-    if (ctl && ctl[0] != 0) return;
-    constexpr int kRows = kSpmvThreads / P;
-    const int j = threadIdx.x % P;
-    const bool jv = j < k;
-    V a[1] = {V(0)};
-    for (int64_t row = blockIdx.x * (int64_t)kRows + threadIdx.x / P; row < num_rows;
-         row += (int64_t)gridDim.x * kRows) {
-        const int64_t s = row_ptrs[row], e = row_ptrs[row + 1];
-        V acc = V(0);
-        constexpr int kB = 4;
-        for (int64_t t = s; t < e; t += kB) {
-            I cc[kB];
-            V vv[kB], xx[kB];
-#pragma unroll
-            for (int u = 0; u < kB; ++u) {
-                cc[u] = t + u < e ? col_idxs[t + u] : I(0);
-                vv[u] = t + u < e ? values[t + u] : V(0);
-            }
-#pragma unroll
-            for (int u = 0; u < kB; ++u) xx[u] = (t + u < e && jv) ? b[(int64_t)cc[u] * k + j] : V(0);
-#pragma unroll
-            for (int u = 0; u < kB; ++u)
-                if (t + u < e) acc += vv[u] * xx[u];
-        }
-        if (jv) {
-            c[row * k + j] = acc;
-            a[0] += b[row * k + j] * acc;
-        }
-    }
-    cta_column_sums<V, P, 1, kSpmvThreads>(a, red);
-    if (!grid_column_sums<V, 1, kSpmvThreads>(a, k, partials, counter, tot, &is_last)) return;
-    if (threadIdx.x < k) dots[threadIdx.x] = tot[0][threadIdx.x];
-}
+using namespace mrhs;   // layout, grids, column sums, the SpMV (fused_mrhs.cuh)
 
 template <typename V, int P>
 __global__ void __launch_bounds__(kThreads)
@@ -275,15 +145,6 @@ __global__ void init_scalars_kernel(int64_t k, V* sc, uint8_t* status, int32_t* 
 }
 
 // ---- host side of the entry points ----------------------------------------------------------------
-#define B200_FCGM_BY_LANES(P, CALL) \
-    switch (P) {                    \
-    case 2: CALL(2); break;         \
-    case 4: CALL(4); break;         \
-    case 8: CALL(8); break;         \
-    case 16: CALL(16); break;       \
-    default: CALL(32); break;       \
-    }
-
 template <typename V, bool INIT>
 b200_status step_xr(b200_ctx* ctx, int64_t n, int64_t k, V* x, V* r, const V* p, const V* q, V* z,
                     const V* inv_diag, V* sc, uint8_t* status, int32_t* ctl, V* work, int baseline, V factor)
@@ -295,7 +156,7 @@ b200_status step_xr(b200_ctx* ctx, int64_t n, int64_t k, V* x, V* r, const V* p,
     step_xr_kernel<V, PP, INIT><<<grid, kThreads, 0, ctx->stream>>>(n, k, x, r, p, q, z, inv_diag, sc, \
                                                                     status, ctl, partials,            \
                                                                     ctx->counters + 2, baseline, factor)
-    B200_FCGM_BY_LANES(P, B200_XR)
+    B200_MRHS_BY_LANES(P, B200_XR)
 #undef B200_XR
     B200_LAUNCH_CHECK(ctx);
     return B200_OK;
@@ -328,31 +189,8 @@ b200_status step_p(b200_ctx* ctx, int64_t n, int64_t k, V* p, const V* z, const 
     const int P = lanes_for(k);
     const int grid = rows_grid<kThreads>(n, P, step_cap(ctx));
 #define B200_P(PP) step_p_kernel<V, PP><<<grid, kThreads, 0, ctx->stream>>>(n, k, p, z, sc, status, ctl)
-    B200_FCGM_BY_LANES(P, B200_P)
+    B200_MRHS_BY_LANES(P, B200_P)
 #undef B200_P
-    B200_LAUNCH_CHECK(ctx);
-    return B200_OK;
-}
-
-template <typename V, typename I>
-b200_status spmv_mdot(b200_ctx* ctx, int64_t num_rows, int64_t num_cols, int64_t nnz, const I* row_ptrs,
-                      const I* col_idxs, const V* values, const V* b, int64_t k, V* c, V* dots, V* work,
-                      const int32_t* ctl)
-{
-    B200_REQUIRE(ctx && dots && work, "null argument");
-    B200_REQUIRE(num_rows >= 0 && num_cols >= 0 && nnz >= 0, "negative size");
-    B200_REQUIRE(k >= 2 && k <= kMaxCols, "k must be in [2, 32]");
-    B200_REQUIRE(num_rows == 0 || (row_ptrs && c && b), "null pointer");
-    B200_REQUIRE(nnz == 0 || (col_idxs && values), "null pointer");
-    const int P = lanes_for(k);
-    // no rows: one CTA still runs and writes zero dots
-    const int grid = rows_grid<kSpmvThreads>(num_rows, P, spmv_cap(ctx));
-#define B200_MD(PP)                                                                                   \
-    spmv_mdot_kernel<V, I, PP><<<grid, kSpmvThreads, 0, ctx->stream>>>(num_rows, k, row_ptrs, col_idxs, \
-                                                                       values, b, c, dots, work,        \
-                                                                       ctx->counters + 1, ctl)
-    B200_FCGM_BY_LANES(P, B200_MD)
-#undef B200_MD
     B200_LAUNCH_CHECK(ctx);
     return B200_OK;
 }
@@ -403,8 +241,9 @@ B200_DEF_FCGM(f32, float)
                                              const VT* values, const VT* b, int64_t k, VT* c,        \
                                              VT* dots, VT* work, const int32_t* ctl)                 \
     {                                                                                                \
-        return b200::fcgm::spmv_mdot<VT, IT>(ctx, num_rows, num_cols, nnz, row_ptrs, col_idxs, values, \
-                                             b, k, c, dots, work, ctl);                              \
+        return b200::mrhs::spmv_mdot<VT, IT, b200::mrhs::DotB>(ctx, num_rows, num_cols, nnz, row_ptrs, \
+                                                               col_idxs, values, b, k, c, nullptr, dots, \
+                                                               nullptr, work, ctl);                     \
     }
 
 B200_DEF_SPMV_MDOT(f64, double, i32, int32_t)

@@ -95,6 +95,8 @@ std::unique_ptr<LinOp> make_solver(std::shared_ptr<Executor> exec, int kind,
         auto f = solver::Bicgstab<V>::build();
         // bit 1 of `fused`: the fused BiCGStab iteration is opt-in, bit 0 keeps meaning Cg's
         f.with_criteria(crit).with_fused((fused & 2) != 0).with_check_every(check_every);
+        // bit 4 of `fused`: its iteration for several right-hand sides, opt-in as well
+        f.with_fused_multi_rhs((fused & 16) != 0);
         set_pre(f);
         return f.on(exec)->generate(A);
     }

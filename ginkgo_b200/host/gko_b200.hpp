@@ -134,6 +134,11 @@ struct viabi;
         static constexpr auto cg_mrhs_init = b200_cg_mrhs_init_##S;                             \
         static constexpr auto cg_mrhs_step_p = b200_cg_mrhs_step_p_##S;                         \
         static constexpr auto cg_mrhs_step_xr = b200_cg_mrhs_step_xr_##S;                       \
+        static constexpr auto bicgstab_mrhs_work_size = b200_bicgstab_mrhs_work_size_##S;       \
+        static constexpr auto bicgstab_mrhs_init = b200_bicgstab_mrhs_init_##S;                 \
+        static constexpr auto bicgstab_mrhs_step_p = b200_bicgstab_mrhs_step_p_##S;             \
+        static constexpr auto bicgstab_mrhs_step_s = b200_bicgstab_mrhs_step_s_##S;             \
+        static constexpr auto bicgstab_mrhs_step_xr = b200_bicgstab_mrhs_step_xr_##S;           \
     };
 GKOB_V(double, f64)
 GKOB_V(float, f32)
@@ -150,6 +155,7 @@ GKOB_V(float, f32)
         static constexpr auto csr_spmv_dot = b200_csr_spmv_dot_##S##_##T;                       \
         static constexpr auto csr_spmv_dot2 = b200_csr_spmv_dot2_##S##_##T;                     \
         static constexpr auto csr_spmv_mdot = b200_csr_spmv_mdot_##S##_##T;                     \
+        static constexpr auto csr_spmv_mdot2 = b200_csr_spmv_mdot2_##S##_##T;                   \
         static constexpr auto csr_extract_diagonal = b200_csr_extract_diagonal_##S##_##T;       \
         static constexpr auto csr_convert_to_ell = b200_csr_convert_to_ell_##S##_##T;           \
         static constexpr auto csr_convert_to_sellp = b200_csr_convert_to_sellp_##S##_##T;       \

@@ -717,6 +717,32 @@ protected:
         }
         return !((((std::uintptr_t)f.A->get_const_col_idxs()) | ((std::uintptr_t)f.A->get_const_values())) & 15);
     }
+    // the several-column fused paths of Cg and Bicgstab keep their workspace, control block and graph
+    // across applies; what the graph bakes in (the index arrays as untyped pointers: int32 or int64)
+    struct MultiRhsKey {
+        int64 k = 0;
+        const V* ws = nullptr;
+        const V* x = nullptr;
+        const V* inv_diag = nullptr;
+        const void* row_ptrs = nullptr;
+        const void* col_idxs = nullptr;
+        const V* values = nullptr;
+        int64 nnz = -1;
+        bool operator==(const MultiRhsKey& o) const
+        {
+            return k == o.k && ws == o.ws && x == o.x && inv_diag == o.inv_diag && row_ptrs == o.row_ptrs &&
+                   col_idxs == o.col_idxs && values == o.values && nnz == o.nnz;
+        }
+    };
+    struct MultiRhsState {
+        std::unique_ptr<Dense> ws;
+        array<V> sc, work;
+        array<uint8> status;
+        array<int32> ctl;
+        int64 n = -1, k = 0;
+        b200_graph* graph = nullptr;
+        MultiRhsKey key;
+    };
     std::shared_ptr<const LinOp> system_matrix_;
     std::shared_ptr<const LinOp> preconditioner_;
     std::vector<std::shared_ptr<const stop::CriterionFactory>> criteria_;
@@ -1069,32 +1095,8 @@ private:
     mutable b200_graph* graph_ = nullptr;
     mutable const V* graph_x_ = nullptr;
     mutable const V* graph_diag_ = nullptr;
-    // what the several-column graph bakes in (the index arrays as untyped pointers: int32 or int64)
-    struct MultiRhsKey {
-        int64 k = 0;
-        const V* ws = nullptr;
-        const V* x = nullptr;
-        const V* inv_diag = nullptr;
-        const void* row_ptrs = nullptr;
-        const void* col_idxs = nullptr;
-        const V* values = nullptr;
-        int64 nnz = -1;
-        bool operator==(const MultiRhsKey& o) const
-        {
-            return k == o.k && ws == o.ws && x == o.x && inv_diag == o.inv_diag && row_ptrs == o.row_ptrs &&
-                   col_idxs == o.col_idxs && values == o.values && nnz == o.nnz;
-        }
-    };
-    struct MultiRhsState {
-        std::unique_ptr<Dense> ws;
-        array<V> sc, work;
-        array<uint8> status;
-        array<int32> ctl;
-        int64 n = -1, k = 0;
-        b200_graph* graph = nullptr;
-        MultiRhsKey key;
-    };
-    mutable MultiRhsState mrhs_;
+    using MultiRhsKey = typename Base::MultiRhsKey;
+    mutable typename Base::MultiRhsState mrhs_;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -1795,11 +1797,19 @@ class Bicgstab : public SolverBase<V> {
 public:
     struct Factory : SolverFactoryBase<Factory> {
         bool fused_ = false;
+        bool fused_multi_rhs_ = false;
         int check_every_ = 16;
         // ginkgo_b200 extension: device-resident fused iteration where applicable (default off)
         Factory& with_fused(bool f)
         {
             fused_ = f;
+            return *this;
+        }
+        // ginkgo_b200 extension: the device-resident iteration for 2..32 right-hand sides, one
+        // matrix pass per SpMV for all columns (opt-in)
+        Factory& with_fused_multi_rhs(bool f)
+        {
+            fused_multi_rhs_ = f;
             return *this;
         }
         Factory& with_check_every(int k)
@@ -1815,11 +1825,16 @@ public:
     };
     static Factory build() { return Factory{}; }
     bool used_fused_path() const { return used_fused_; }
-    ~Bicgstab() override { b200_graph_destroy(graph_); }
+    ~Bicgstab() override
+    {
+        b200_graph_destroy(graph_);
+        b200_graph_destroy(mrhs_.graph);
+    }
 
 protected:
     Bicgstab(std::shared_ptr<const Executor> exec, const Factory& f, std::shared_ptr<const LinOp> op)
-        : Base(exec, f, op), fused_(f.fused_), check_every_(std::max(1, f.check_every_))
+        : Base(exec, f, op), fused_(f.fused_), fused_multi_rhs_(f.fused_multi_rhs_),
+          check_every_(std::max(1, f.check_every_))
     {}
     using Base::apply_impl;
     void apply_impl(const LinOp* lb, LinOp* lx) const override
@@ -1828,6 +1843,8 @@ protected:
         auto x = as<Dense>(lx);
         if (fused_ && try_fused<int32>(b, x)) return;
         if (fused_ && try_fused<int64>(b, x)) return;
+        if (fused_multi_rhs_ && try_fused_multi_rhs<int32>(b, x)) return;
+        if (fused_multi_rhs_ && try_fused_multi_rhs<int64>(b, x)) return;
         used_fused_ = false;
         auto exec = this->exec_;
         auto ctx = exec->ctx();
@@ -1972,8 +1989,97 @@ protected:
         return true;
     }
 
+    // Fused device-resident path for k = 2..32 right-hand sides (csrc/fused_bicgstab_mrhs.cu): the
+    // admission of try_fused with b and x of k columns stored without gaps.  Every column stops on
+    // its own, at the top or the mid-iteration check; the device keeps a stopped column's x, r and p
+    // as the loop's masked steps leave them, and the host reads all k statuses at the end.
+    template <typename I>
+    bool try_fused_multi_rhs(const Dense* b, Dense* x) const
+    {
+        typename Base::template FusedProblem<I> f;
+        if (b->get_size().cols < 2 || !this->template fused_problem<I>(b, x, f, 32) ||
+            !this->template fused_scalar_preconditioner<I>(f))
+            return false;
+        const auto A = f.A;
+        auto exec = this->exec_;
+        auto ctx = exec->ctx();
+        const int64 n = this->size_.rows;
+        const int64 k = (int64)b->get_size().cols;
+        const int64 nnz = A->get_num_stored_elements();
+        auto& m = mrhs_;
+        // workspace r, rr, p, v, y, s, t, z (n x k each), per-column scalars, statuses, control block,
+        // partials; kept across applies
+        if (!m.ws || m.n != n || m.k != k) {
+            m.ws = Dense::create(exec, dim2{(size_type)(8 * n * k), 1});
+            m.sc = array<V>(exec, (size_type)(10 * k));
+            m.status = array<uint8>(exec, (size_type)k);
+            m.ctl = array<int32>(exec, 8);
+            m.work = array<V>(exec, (size_type)vabi<V>::bicgstab_mrhs_work_size(ctx, k));
+            m.n = n;
+            m.k = k;
+            b200_graph_destroy(m.graph);  // it holds the pointers just freed
+            m.graph = nullptr;
+        }
+        const int64 nk = n * k;
+        V* r = m.ws->get_values();
+        V *rr = r + nk, *p = r + 2 * nk, *v = r + 3 * nk, *y = r + 4 * nk, *s = r + 5 * nk, *t = r + 6 * nk,
+          *z = r + 7 * nk;
+        V* xv = x->get_values();
+        V* sc = m.sc.get_data();
+        uint8* status = m.status.get_data();
+        int32* ctl = m.ctl.get_data();
+        V* work = m.work.get_data();
+        const V* inv_diag = f.inv_diag;
+        // r = b - A x
+        exec->copy(r, b->get_const_values(), nk);
+        auto rview = Dense::create_view(exec, dim2{(size_type)n, (size_type)k}, r, (size_type)k);
+        A->apply(this->neg_one_.get(), x, this->one_.get(), rview.get());
+        if (f.baseline == 0)  // ||b_j|| into sc[4k + j]
+            GKOB_CALL(vabi<V>::norm2(ctx, n, k, b->get_const_values(), k, sc + 4 * k));
+        GKOB_CALL(vabi<V>::bicgstab_mrhs_init(ctx, n, k, r, rr, p, v, y, s, t, z, sc, status, ctl, work,
+                                              f.max_iters, f.res_kind, f.iter_first, f.baseline, (V)f.factor));
+        auto spmv_mdot2 = [&](const V* in, V* out, const V* w, V* dots, V* dots2) {
+            GKOB_CALL((viabi<V, I>::csr_spmv_mdot2(ctx, n, n, nnz, A->get_const_row_ptrs(), A->get_const_col_idxs(),
+                                                   A->get_const_values(), in, k, out, w, dots, dots2, work,
+                                                   ctl)));
+        };
+        // the graph bakes in every pointer and size below: re-capture when one changes
+        const MultiRhsKey key{k, r, xv, inv_diag, A->get_const_row_ptrs(), A->get_const_col_idxs(),
+                              A->get_const_values(), nnz};
+        if (!m.graph || !(m.key == key)) {
+            b200_graph_destroy(m.graph);
+            m.graph = nullptr;
+            GKOB_CALL(b200_graph_begin_capture(ctx));
+            for (int it = 0; it < check_every_; ++it) {
+                GKOB_CALL(vabi<V>::bicgstab_mrhs_step_p(ctx, n, k, p, r, v, y, inv_diag, sc, status, ctl));
+                spmv_mdot2(y, v, rr, sc + 2 * k, nullptr);
+                GKOB_CALL(vabi<V>::bicgstab_mrhs_step_s(ctx, n, k, r, v, s, z, inv_diag, sc, status, ctl, work));
+                spmv_mdot2(z, t, s, sc + 8 * k, sc + 2 * k);
+                GKOB_CALL(vabi<V>::bicgstab_mrhs_step_xr(ctx, n, k, xv, r, s, t, y, z, rr, sc, status, ctl,
+                                                         work));
+            }
+            GKOB_CALL(b200_graph_end_capture(ctx, &m.graph));
+            m.key = key;
+        }
+        // every captured iteration ends with step_xr, so a stop read here has its finalizes paid
+        int32 h[8] = {0};
+        exec->copy_to_host(h, m.ctl.get_const_data(), 8);
+        while (h[0] == 0) {
+            const int32 before = h[1];
+            GKOB_CALL(b200_graph_launch(ctx, m.graph));
+            exec->copy_to_host(h, m.ctl.get_const_data(), 8);
+            if (h[0] == 0 && h[1] == before)
+                throw Error("fused BiCGStab (several right-hand sides): the device iteration made no progress");
+        }
+        this->num_iterations_ = (size_type)h[1];
+        this->status_ = m.status.to_host();
+        used_fused_ = true;
+        return true;
+    }
+
 private:
     bool fused_;
+    bool fused_multi_rhs_;
     int check_every_;
     mutable bool used_fused_ = false;
     mutable std::unique_ptr<Dense> ws_;
@@ -1983,6 +2089,8 @@ private:
     mutable b200_graph* graph_ = nullptr;
     mutable const V* graph_x_ = nullptr;
     mutable const V* graph_diag_ = nullptr;
+    using MultiRhsKey = typename Base::MultiRhsKey;
+    mutable typename Base::MultiRhsState mrhs_;
 };
 
 // ---------------------------------------------------------------------------------------------

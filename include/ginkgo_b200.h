@@ -760,6 +760,77 @@ B200_DECL_SPMV_MDOT(f32, float, i32, int32_t)
 B200_DECL_SPMV_MDOT(f32, float, i64, int64_t)
 
 /* ---------------------------------------------------------------------------
+ * Fused BiCGStab iteration for k = 2..32 right-hand sides (ginkgo_b200 extension behind
+ * solver::Bicgstab::apply with with_fused_multi_rhs(true), single GPU).  The regrouping of the fused
+ * BiCGStab above with every vector n x k row-major (stride k) and every scalar per column; each SpMV
+ * is one matrix pass for all columns.  The element-wise steps of a stopped column are skipped, as the
+ * reference's bicgstab::step_1/2/3 skip them by the column's stopping_status
+ * (reference/solver/bicgstab_kernels.cpp:65-178); d = inv_diag of a scalar Jacobi preconditioner,
+ * NULL for Identity:
+ *   step_p     p_j = r_j + (rho_j/prev_rho_j*alpha_j/omega_j)(p_j - omega_j v_j),
+ *              p_j = r_j if prev_rho_j*omega_j == 0; y_j = d.p_j     (bicgstab::step_1 + jacobi apply)
+ *   spmv_mdot2 v = A y for all columns, beta_j = rr_j . v_j        (Csr::apply + compute_conj_dot)
+ *   step_s     alpha_j = rho_j/beta_j (0 and s_j = r_j if beta_j == 0); s_j = r_j - alpha_j v_j;
+ *              z_j = d.s_j; ||s_j||^2; the mid-iteration check of every running column, which does
+ *              not set the finalized bit     (bicgstab::step_2 + norm2 + criterion check + jacobi apply)
+ *   spmv_mdot2 t = A z, gamma_j = s_j . t_j and beta_j = t_j . t_j (Csr::apply + 2 compute_conj_dot)
+ *   step_xr    omega_j = gamma_j/beta_j (0 if beta_j == 0); x_j += alpha_j y_j + omega_j z_j;
+ *              r_j = s_j - omega_j t_j; rho_j = rr_j . r_j; ||r_j||^2; rho / prev_rho shifted; the
+ *              top-of-iteration check of every running column; a column stopped at this iteration's
+ *              mid check gets only x_j += alpha_j y_j and its finalized bit
+ *                                 (bicgstab::step_3 + finalize + dot + norm2 + criterion check)
+ *   init       r holds b - A x; rr = r; p = v = y = s = t = z = 0; rho = prev_rho = alpha = beta =
+ *              gamma = omega = 1; all columns running; rho, ||r||^2, each column's baseline and the
+ *              first check                              (bicgstab::initialize + dot + norm2 + check)
+ * sc:     VT[10k]   sc[s*k + j]: s = 0 rho, 1 prev_rho, 2 beta (rr.v, then t.t), 3 ||r||^2, 4 tau0,
+ *                   5 threshold, 6 alpha, 7 omega, 8 gamma, 9 ||s||^2
+ * status: uint8[k]  stopping_status byte of every column (0 = running)
+ * ctl:    int32[8]  0 nonzero once every column has stopped, 1 iterations, 2 max_iters,
+ *                   3 res_kind (0 none, 1 ResidualNorm, 2 ImplicitResidualNorm), 4 iter_first,
+ *                   5 some column stopped at the mid check and owes its finalize
+ * Once ctl[0] != 0 and ctl[5] == 0 every kernel is a no-op, so graphs of several iterations can be
+ * replayed and the host polls ctl after each; every iteration ends with step_xr, which pays what a
+ * mid-check stop owes.  `work` has b200_bicgstab_mrhs_work_size(k) elements.  baseline: 0 rhs_norm
+ * (caller stores ||b_j|| in sc[4k + j] first), 1 initial_resnorm, 2 absolute.
+ *
+ * b200_csr_spmv_mdot2: c = A b for the k columns of the row-major b, c and w (stride k), dots[j] =
+ * w_j . c_j and, unless dots2 is NULL, dots2[j] = c_j . c_j.  c is bit-identical to b200_csr_spmv
+ * with num_rhs = k; the sums are added in a fixed order.  ctl may be NULL; with num_rows == 0 both
+ * sums are 0.  No plan and no alignment are required.
+ * ------------------------------------------------------------------------- */
+#define B200_DECL_FBICGSTABM(V, VT)                                                            \
+    int64_t b200_bicgstab_mrhs_work_size_##V(const b200_ctx* ctx, int64_t k);                  \
+    b200_status b200_bicgstab_mrhs_init_##V(b200_ctx* ctx, int64_t n, int64_t k, const VT* r,  \
+                                            VT* rr, VT* p, VT* v, VT* y, VT* s, VT* t, VT* z,  \
+                                            VT* sc, uint8_t* status, int32_t* ctl, VT* work,   \
+                                            int64_t max_iters, int32_t res_kind,               \
+                                            int32_t iter_first, int32_t baseline,              \
+                                            VT reduction_factor);                              \
+    b200_status b200_bicgstab_mrhs_step_p_##V(b200_ctx* ctx, int64_t n, int64_t k, VT* p,      \
+                                              const VT* r, const VT* v, VT* y,                 \
+                                              const VT* inv_diag, const VT* sc,                \
+                                              const uint8_t* status, const int32_t* ctl);      \
+    b200_status b200_bicgstab_mrhs_step_s_##V(b200_ctx* ctx, int64_t n, int64_t k, const VT* r, \
+                                              const VT* v, VT* s, VT* z, const VT* inv_diag,   \
+                                              VT* sc, uint8_t* status, int32_t* ctl, VT* work); \
+    b200_status b200_bicgstab_mrhs_step_xr_##V(b200_ctx* ctx, int64_t n, int64_t k, VT* x,     \
+                                               VT* r, const VT* s, const VT* t, const VT* y,   \
+                                               const VT* z, const VT* rr, VT* sc,              \
+                                               uint8_t* status, int32_t* ctl, VT* work);
+#define B200_DECL_SPMV_MDOT2(V, VT, I, IT)                                                     \
+    b200_status b200_csr_spmv_mdot2_##V##_##I(                                                 \
+        b200_ctx* ctx, int64_t num_rows, int64_t num_cols, int64_t nnz, const IT* row_ptrs,    \
+        const IT* col_idxs, const VT* values, const VT* b, int64_t k, VT* c, const VT* w,      \
+        VT* dots, VT* dots2, VT* work, const int32_t* ctl);
+
+B200_DECL_FBICGSTABM(f64, double)
+B200_DECL_FBICGSTABM(f32, float)
+B200_DECL_SPMV_MDOT2(f64, double, i32, int32_t)
+B200_DECL_SPMV_MDOT2(f64, double, i64, int64_t)
+B200_DECL_SPMV_MDOT2(f32, float, i32, int32_t)
+B200_DECL_SPMV_MDOT2(f32, float, i64, int64_t)
+
+/* ---------------------------------------------------------------------------
  * Fused GMRES iteration, modified Gram-Schmidt (ginkgo_b200 extension behind solver::Gmres::apply
  * with with_fused(true), single GPU; it regroups one iteration of core/solver/gmres.cpp:453-530 at
  * Krylov index j -- criterion check, preconditioner, SpMV, j+1 dots and sub_scaled, norm2,
