@@ -155,6 +155,8 @@ std::unique_ptr<LinOp> make_solver(std::shared_ptr<Executor> exec, int kind,
     f.with_criteria(crit).with_krylov_dim((size_type)krylov_dim);
     // bit 2 of `fused`: the fused GMRES iteration is opt-in, as BiCGStab's
     f.with_fused((fused & 4) != 0).with_check_every(check_every);
+    // bit 5: the fused GMRES iteration for 2..32 right-hand sides, opt-in and independent of bit 2
+    f.with_fused_multi_rhs((fused & 32) != 0);
     f.with_ortho_method(ortho == 0   ? solver::gmres::ortho_method::mgs
                         : ortho == 1 ? solver::gmres::ortho_method::cgs
                                      : solver::gmres::ortho_method::cgs2);

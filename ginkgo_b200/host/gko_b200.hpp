@@ -139,6 +139,13 @@ struct viabi;
         static constexpr auto bicgstab_mrhs_step_p = b200_bicgstab_mrhs_step_p_##S;             \
         static constexpr auto bicgstab_mrhs_step_s = b200_bicgstab_mrhs_step_s_##S;             \
         static constexpr auto bicgstab_mrhs_step_xr = b200_bicgstab_mrhs_step_xr_##S;           \
+        static constexpr auto gmres_mrhs_work_size = b200_gmres_mrhs_work_size_##S;             \
+        static constexpr auto gmres_mrhs_init = b200_gmres_mrhs_init_##S;                       \
+        static constexpr auto gmres_mrhs_scale = b200_gmres_mrhs_scale_##S;                     \
+        static constexpr auto gmres_mrhs_mgs_pass = b200_gmres_mrhs_mgs_pass_##S;               \
+        static constexpr auto gmres_mrhs_multi_dot = b200_gmres_mrhs_multi_dot_##S;             \
+        static constexpr auto gmres_mrhs_sub_pass = b200_gmres_mrhs_sub_pass_##S;               \
+        static constexpr auto gmres_mrhs_final_pass = b200_gmres_mrhs_final_pass_##S;           \
     };
 GKOB_V(double, f64)
 GKOB_V(float, f32)

@@ -2123,7 +2123,15 @@ public:
             fused_ = f;
             return *this;
         }
-        // iterations per graph launch (and per read of the control block) on the fused path
+        bool fused_multi_rhs_ = false;
+        // ginkgo_b200 extension: the device-resident iteration for 2..32 right-hand sides, one matrix
+        // pass per SpMV for all columns (opt-in, independent of with_fused)
+        Factory& with_fused_multi_rhs(bool f)
+        {
+            fused_multi_rhs_ = f;
+            return *this;
+        }
+        // iterations per graph launch (and per read of the control block) on the fused paths
         Factory& with_check_every(int k)
         {
             check_every_ = k;
@@ -2137,12 +2145,16 @@ public:
     };
     static Factory build() { return Factory{}; }
     bool used_fused_path() const { return used_fused_; }
-    ~Gmres() override { drop_graphs(); }
+    ~Gmres() override
+    {
+        drop_graphs();
+        drop_mrhs_graphs();
+    }
 
 protected:
     Gmres(std::shared_ptr<const Executor> exec, const Factory& f, std::shared_ptr<const LinOp> op)
         : Base(exec, f, op), krylov_dim_(f.krylov_dim_), ortho_(f.ortho_), fused_(f.fused_),
-          check_every_(std::max(1, f.check_every_))
+          fused_multi_rhs_(f.fused_multi_rhs_), check_every_(std::max(1, f.check_every_))
     {}
     using Base::apply_impl;
     void apply_impl(const LinOp* lb, LinOp* lx) const override
@@ -2151,6 +2163,8 @@ protected:
         auto x = as<Dense>(lx);
         if (fused_ && try_fused<int32>(b, x)) return;
         if (fused_ && try_fused<int64>(b, x)) return;
+        if (fused_multi_rhs_ && try_fused_multi_rhs<int32>(b, x)) return;
+        if (fused_multi_rhs_ && try_fused_multi_rhs<int64>(b, x)) return;
         used_fused_ = false;
         auto exec = this->exec_;
         auto ctx = exec->ctx();
@@ -2454,10 +2468,176 @@ protected:
         graphs_.clear();
     }
 
+    // Fused device-resident path for k = 2..32 right-hand sides (csrc/fused_gmres_mrhs.cu): at Krylov
+    // index j, MGS takes j + 3 launches, CGS 4 and CGS2 6, and the k-wide SpMV is one matrix pass for all
+    // columns.  Every array the restart block shares with the loop kernels has the loop's layout, so the
+    // initial residual, the restart and the final update are the loop's own calls on all k columns.  Each
+    // column stops on its own; a batch of check_every iterations per graph never crosses a restart.
+    template <typename I>
+    bool try_fused_multi_rhs(const Dense* b, Dense* x) const
+    {
+        if (krylov_dim_ == 0) return false;
+        typename Base::template FusedProblem<I> f;
+        // ImplicitResidualNorm: the loop reports NotSupported, and so must this solver
+        if (b->get_size().cols < 2 || !this->template fused_problem<I>(b, x, f, 32) || f.res_kind == 2)
+            return false;
+        // Identity or scalar Jacobi of either index type.  Block Jacobi is the loop's: its k-column apply
+        // switches to a tensor-core kernel whose bits a SIMT apply would not reproduce.
+        const V* inv_diag = nullptr;
+        const LinOp* pre = this->preconditioner_.get();
+        if (auto J = dynamic_cast<const preconditioner::Jacobi<V, int32>*>(pre)) {
+            if (J->get_max_block_size() != 1) return false;
+            inv_diag = J->get_blocks();
+        } else if (auto J = dynamic_cast<const preconditioner::Jacobi<V, int64>*>(pre)) {
+            if (J->get_max_block_size() != 1) return false;
+            inv_diag = J->get_blocks();
+        } else if (!dynamic_cast<const matrix::Identity<V>*>(pre)) {
+            return false;
+        }
+        const auto A = f.A;
+        auto exec = this->exec_;
+        auto ctx = exec->ctx();
+        const int64 n = this->size_.rows, kd = (int64)krylov_dim_;
+        const int64 k = (int64)b->get_size().cols, nk = n * k;
+        const int64 nnz = A->get_num_stored_elements();
+        auto& m = mrhs_;
+        // basis n (kd+1) x k; residual, z, before, after n x k each; the Hessenberg kd x (kd+1) k;
+        // sc[3k], gsin, gcos, y (kd x k), rnc, haux ((kd+1) x k), rnorm; kept across applies
+        if (!m.ws || m.n != n || m.k != k) {
+            m.ws = Dense::create(exec, dim2{(size_type)(nk * (kd + 5)), 1});
+            mhess_ = Dense::create(exec, dim2{(size_type)kd, (size_type)((kd + 1) * k)});
+            m.sc = array<V>(exec, (size_type)(k * (5 * kd + 6)));
+            m.status = array<uint8>(exec, (size_type)k);
+            m.ctl = array<int32>(exec, 8);
+            m.work = array<V>(exec, (size_type)vabi<V>::gmres_mrhs_work_size(ctx, k, kd));
+            mfin_ = array<std::uint64_t>(exec, (size_type)k);
+            m.n = n;
+            m.k = k;
+            drop_mrhs_graphs();  // they hold the pointers just freed
+        }
+        V* K = m.ws->get_values();
+        auto vec = [&](int c) {
+            return Dense::create_view(exec, dim2{(size_type)n, (size_type)k}, K + nk * (kd + 1 + c), (size_type)k);
+        };
+        auto residual = vec(0), z = vec(1), before = vec(2), after = vec(3);
+        V* hess = mhess_->get_values();
+        const int64 hs = mhess_->get_stride();
+        V *sc = m.sc.get_data(), *gsin = sc + 3 * k, *gcos = gsin + kd * k, *rnc = gcos + kd * k,
+          *y = rnc + (kd + 1) * k, *rnorm = y + kd * k, *haux = rnorm + k;
+        auto rnorm_view = Dense::create_view(exec, dim2{1, (size_type)k}, rnorm, (size_type)k);
+        std::uint64_t* fin = mfin_.get_data();
+        uint8* status = m.status.get_data();
+        int32* ctl = m.ctl.get_data();
+        V* work = m.work.get_data();
+        // the loop's start: fresh Hessenberg, rnc, y and haux; initialize; r = b - A x; ||r||; restart
+        mhess_->fill(V(0));
+        GKOB_CALL(vabi<V>::fill(ctx, (3 * kd + 3) * k, 1, rnc, 1, V(0)));
+        GKOB_CALL(vabi<V>::gmres_initialize(ctx, n, k, kd, b->get_const_values(), k, residual->get_values(), k, gsin,
+                                            k, gcos, k, status));
+        this->system_matrix_->apply(this->neg_one_.get(), x, this->one_.get(), residual.get());
+        residual->compute_norm2(rnorm_view.get());
+        auto restart = [&] {
+            GKOB_CALL(vabi<V>::gmres_restart(ctx, n, k, residual->get_const_values(), k, rnorm, rnc, K, k, fin));
+        };
+        restart();
+        if (f.baseline == 0)  // ||b_c|| into sc[k + c]
+            GKOB_CALL(vabi<V>::norm2(ctx, n, k, b->get_const_values(), k, sc + k));
+        GKOB_CALL(vabi<V>::gmres_mrhs_init(ctx, k, rnorm, sc, status, ctl, f.max_iters, f.res_kind, f.iter_first,
+                                           f.baseline, (V)f.factor));
+        // before keeps a finalized column's last correction, as the loop's does
+        auto solve_and_update = [&] {
+            GKOB_CALL(vabi<V>::gmres_solve_krylov(ctx, k, rnc, k, hess, hs, y, k, fin, status));
+            GKOB_CALL(vabi<V>::gmres_multi_axpy(ctx, n, k, K, k, y, k, before->get_values(), k, fin, status));
+            this->preconditioner_->apply(before.get(), after.get());
+            x->add_scaled(this->one_.get(), after.get());
+        };
+        auto enqueue_iteration = [&](int64 j) {
+            V *vj = K + j * nk, *w = vj + nk, *hcol = hess + j * hs;
+            V* in = vj;
+            if (inv_diag) {
+                GKOB_CALL(vabi<V>::gmres_mrhs_scale(ctx, n, k, vj, z->get_values(), inv_diag, sc, status, ctl, j > 0));
+                in = z->get_values();
+            } else if (j > 0) {
+                GKOB_CALL(vabi<V>::gmres_mrhs_scale(ctx, n, k, vj, nullptr, nullptr, sc, status, ctl, 1));
+            }
+            GKOB_CALL((viabi<V, I>::csr_spmv_mdot2(ctx, n, n, nnz, A->get_const_row_ptrs(), A->get_const_col_idxs(),
+                                                   A->get_const_values(), in, k, w, K, hcol, nullptr, work, ctl)));
+            auto final_pass = [&](int64 first, const V* coef, const V* add) {
+                GKOB_CALL(vabi<V>::gmres_mrhs_final_pass(ctx, n, k, w, K, first, coef, add, hcol, j, gsin, gcos,
+                                                         rnorm, rnc, fin, status, sc, ctl, work));
+            };
+            if (ortho_ == gmres::ortho_method::mgs) {
+                for (int64 i = 1; i <= j; ++i)
+                    GKOB_CALL(vabi<V>::gmres_mrhs_mgs_pass(ctx, n, k, w, K + (i - 1) * nk, K + i * nk, hcol, i,
+                                                           status, ctl, work));
+                final_pass(j, hcol, nullptr);
+                return;
+            }
+            // CGS: h_1..h_j in one pass (h_0 came with the SpMV), one subtract pass over all bases
+            if (j > 0)
+                GKOB_CALL(vabi<V>::gmres_mrhs_multi_dot(ctx, n, k, j, kd, K + nk, w, hcol + k, status, ctl, work));
+            if (ortho_ == gmres::ortho_method::cgs) {
+                final_pass(0, hcol, nullptr);
+                return;
+            }
+            // CGS2: subtract, re-orthogonalise against all bases into haux, subtract again; h += haux
+            GKOB_CALL(vabi<V>::gmres_mrhs_sub_pass(ctx, n, k, w, K, hcol, j, status, ctl));
+            GKOB_CALL(vabi<V>::gmres_mrhs_multi_dot(ctx, n, k, j + 1, kd, K, w, haux, status, ctl, work));
+            final_pass(0, haux, haux);
+        };
+        // the graphs bake in every pointer and size below: re-capture when one changes.  Batches start at
+        // Krylov index 0, c, 2c, ... and end at the restart.
+        const MultiRhsKey key{k, K, nullptr, inv_diag, A->get_const_row_ptrs(), A->get_const_col_idxs(),
+                              A->get_const_values(), nnz};
+        const int64 ce = std::min<int64>(check_every_, kd);
+        if (mgraphs_.empty() || !(m.key == key)) {
+            drop_mrhs_graphs();
+            for (int64 j0 = 0; j0 < kd; j0 += ce) {
+                b200_graph* g = nullptr;
+                GKOB_CALL(b200_graph_begin_capture(ctx));
+                for (int64 j = j0; j < std::min(j0 + ce, kd); ++j) enqueue_iteration(j);
+                GKOB_CALL(b200_graph_end_capture(ctx, &g));
+                mgraphs_.push_back(g);
+            }
+            m.key = key;
+        }
+        int32 h[8] = {0};
+        exec->copy_to_host(h, ctl, 8);
+        int64 j = 0;
+        while (h[0] == 0) {
+            // the loop's restart on all k columns, only once the check at the top of iteration krylov_dim
+            // said "running"
+            if (j == kd) {
+                solve_and_update();
+                residual->copy_from(b);
+                this->system_matrix_->apply(this->neg_one_.get(), x, this->one_.get(), residual.get());
+                residual->compute_norm2(rnorm_view.get());
+                restart();
+                j = 0;
+            }
+            const int32 before_iters = h[1];
+            GKOB_CALL(b200_graph_launch(ctx, mgraphs_[j / ce]));
+            j = std::min(j + ce, kd);
+            exec->copy_to_host(h, ctl, 8);
+            if (h[0] == 0 && h[1] == before_iters)
+                throw Error("fused GMRES (several right-hand sides): the device iteration made no progress");
+        }
+        solve_and_update();
+        this->record((size_type)h[1], m.status);
+        used_fused_ = true;
+        return true;
+    }
+    void drop_mrhs_graphs() const
+    {
+        for (auto g : mgraphs_) b200_graph_destroy(g);
+        mgraphs_.clear();
+    }
+
 private:
     size_type krylov_dim_;
     gmres::ortho_method ortho_;
     bool fused_;
+    bool fused_multi_rhs_;
     int check_every_;
     mutable bool used_fused_ = false;
     mutable std::unique_ptr<Dense> fkrylov_, fvec_, fhess_;
@@ -2469,6 +2649,12 @@ private:
     mutable std::vector<b200_graph*> graphs_;
     static constexpr int kGraphKey = 7;
     mutable const void* graph_key_[kGraphKey] = {};
+    // the several-column path: workspace and control block in mrhs_, one graph per batch in mgraphs_
+    using MultiRhsKey = typename Base::MultiRhsKey;
+    mutable typename Base::MultiRhsState mrhs_;
+    mutable std::unique_ptr<Dense> mhess_;
+    mutable array<std::uint64_t> mfin_;
+    mutable std::vector<b200_graph*> mgraphs_;
 };
 
 }  // namespace solver

@@ -898,6 +898,64 @@ B200_DECL_SPMV_MDOT2(f32, float, i64, int64_t)
 
 B200_DECL_FGMRES(f64, double)
 B200_DECL_FGMRES(f32, float)
+
+/* ---------------------------------------------------------------------------
+ * Fused GMRES iteration for k = 2..32 right-hand sides (ginkgo_b200 extension behind
+ * solver::Gmres::apply with with_fused_multi_rhs(true), single GPU): the entries above with every
+ * vector n x k row-major (stride k) and every Hessenberg entry, Givens rotation and residual estimate
+ * per column, in the loop's layout -- krylov n (kd+1) x k (basis i, column c at (i n + r) k + c),
+ * hcol row j of the kd x (kd+1) k Hessenberg (h_i of column c at hcol[i k + c]), gsin, gcos, rnc,
+ * haux, rnorm, fin of stride k -- so that the loop's initialize / restart / solve_krylov /
+ * multi_axpy run on them with nrhs = k.  The SpMV is b200_csr_spmv_mdot2 with w = basis 0 and dots =
+ * hcol (h_0), dots2 = NULL; it computes every column.  Every other kernel skips a stopped column:
+ *   scale        v_j = w / sc[c] if `divide`; z = inv_diag . v_j unless inv_diag is NULL
+ *   mgs_pass i   w -= h_{i-1} v_{i-1} (skipped for h == 0); h_i = v_i . w, i = 1..j
+ *   multi_dot    hcol[i k + c] = v_i . w for i < num_bases (<= krylov_dim + 1), one pass over the
+ *                bases for all columns
+ *   sub_pass     w -= coef_i v_i, i = 0..j in basis order (CGS2's first subtraction)
+ *   final_pass   w -= coef_i v_i for i = first..j; h_{j+1} = ||w||, kept in sc[c]; with haux !=
+ *                NULL first h_i += haux_i, i <= j; the Givens update of hessenberg_qr for column c
+ *                with iteration j; the criteria on tau_c = rnorm[c] = |rnc_c[j+1]| for the top of
+ *                iteration j+1
+ *   init         rnorm holds ||b_c - A x_c||; v_0, rnc, fin, gsin, gcos are set by the loop's
+ *                initialize / restart; sets the baselines (sc[k + c] preset to ||b_c|| for
+ *                rhs_norm), the thresholds, the statuses and runs the iteration-0 check
+ * sc:     VT[3k]    sc[s*k + c]: s = 0 ||w|| of the last final pass, 1 tau0, 2 threshold
+ * status: uint8[k]  stopping_status byte of every column (0 = running), WITHOUT the finalized bit
+ * ctl:    int32[8]  0 nonzero once every column has stopped, 1 iterations, 2 max_iters (-1 none),
+ *                   3 res_kind (0 none, 1 ResidualNorm), 4 iter_first
+ * With ctl[0] != 0 every kernel but init is a no-op.  `work` has b200_gmres_mrhs_work_size(k,
+ * krylov_dim) elements; the passes take ticket 2, the multi-dot ticket 3.
+ * ------------------------------------------------------------------------- */
+#define B200_DECL_FGMRESM(V, VT)                                                               \
+    int64_t b200_gmres_mrhs_work_size_##V(const b200_ctx* ctx, int64_t k, int64_t krylov_dim); \
+    b200_status b200_gmres_mrhs_init_##V(b200_ctx* ctx, int64_t k, const VT* rnorm, VT* sc,    \
+                                         uint8_t* status, int32_t* ctl, int64_t max_iters,     \
+                                         int32_t res_kind, int32_t iter_first,                 \
+                                         int32_t baseline, VT reduction_factor);               \
+    b200_status b200_gmres_mrhs_scale_##V(b200_ctx* ctx, int64_t n, int64_t k, VT* v, VT* z,   \
+                                          const VT* inv_diag, const VT* sc,                    \
+                                          const uint8_t* status, const int32_t* ctl,           \
+                                          int32_t divide);                                     \
+    b200_status b200_gmres_mrhs_mgs_pass_##V(b200_ctx* ctx, int64_t n, int64_t k, VT* w,       \
+                                             const VT* v_prev, const VT* v_i, VT* hcol,        \
+                                             int64_t i, const uint8_t* status,                 \
+                                             const int32_t* ctl, VT* work);                    \
+    b200_status b200_gmres_mrhs_multi_dot_##V(b200_ctx* ctx, int64_t n, int64_t k,             \
+                                              int64_t num_bases, int64_t krylov_dim,           \
+                                              const VT* krylov, const VT* w, VT* hcol,         \
+                                              const uint8_t* status, const int32_t* ctl,       \
+                                              VT* work);                                       \
+    b200_status b200_gmres_mrhs_sub_pass_##V(b200_ctx* ctx, int64_t n, int64_t k, VT* w,       \
+                                             const VT* krylov, const VT* coef, int64_t j,      \
+                                             const uint8_t* status, const int32_t* ctl);       \
+    b200_status b200_gmres_mrhs_final_pass_##V(                                                \
+        b200_ctx* ctx, int64_t n, int64_t k, VT* w, const VT* krylov, int64_t first,           \
+        const VT* coef, const VT* haux, VT* hcol, int64_t j, VT* gsin, VT* gcos, VT* rnorm,    \
+        VT* rnc, uint64_t* fin, uint8_t* status, VT* sc, int32_t* ctl, VT* work);
+
+B200_DECL_FGMRESM(f64, double)
+B200_DECL_FGMRESM(f32, float)
 B200_DECL_FGMRES_BLOCK(f64, double, i32, int32_t)
 B200_DECL_FGMRES_BLOCK(f64, double, i64, int64_t)
 B200_DECL_FGMRES_BLOCK(f32, float, i32, int32_t)
