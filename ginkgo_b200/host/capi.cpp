@@ -108,7 +108,8 @@ std::unique_ptr<LinOp> make_solver(std::shared_ptr<Executor> exec, int kind,
     }
     if (kind == 9) {
         auto f = solver::Minres<V>::build();
-        f.with_criteria(crit);
+        // bit 6 of `fused`: the fused MINRES iteration is opt-in, as BiCGStab's and GMRES's
+        f.with_criteria(crit).with_fused((fused & 64) != 0).with_check_every(check_every);
         set_pre(f);
         return f.on(exec)->generate(A);
     }
@@ -633,9 +634,11 @@ int gkob_csr_kernel_variant(void* csr)
             auto cg = dynamic_cast<solver::Cg<V>*>(op);                                         \
             auto bicgstab = dynamic_cast<solver::Bicgstab<V>*>(op);                             \
             auto gmres = dynamic_cast<solver::Gmres<V>*>(op);                                   \
+            auto minres = dynamic_cast<solver::Minres<V>*>(op);                                 \
             *used_fused = cg         ? (int)cg->used_fused_path()                               \
                           : bicgstab ? (int)bicgstab->used_fused_path()                         \
                           : gmres    ? (int)gmres->used_fused_path()                            \
+                          : minres   ? (int)minres->used_fused_path()                           \
                                      : 0;                                                       \
         });                                                                                     \
     }                                                                                           \

@@ -123,6 +123,10 @@ struct viabi;
         static constexpr auto bicgstab_fused_step_p = b200_bicgstab_fused_step_p_##S;           \
         static constexpr auto bicgstab_fused_step_s = b200_bicgstab_fused_step_s_##S;           \
         static constexpr auto bicgstab_fused_step_xr = b200_bicgstab_fused_step_xr_##S;         \
+        static constexpr auto minres_fused_work_size = b200_minres_fused_work_size_##S;         \
+        static constexpr auto minres_fused_init = b200_minres_fused_init_##S;                   \
+        static constexpr auto minres_fused_lanczos = b200_minres_fused_lanczos_##S;             \
+        static constexpr auto minres_fused_update = b200_minres_fused_update_##S;               \
         static constexpr auto gmres_fused_work_size = b200_gmres_fused_work_size_##S;           \
         static constexpr auto gmres_fused_init = b200_gmres_fused_init_##S;                     \
         static constexpr auto gmres_fused_scale = b200_gmres_fused_scale_##S;                   \
@@ -161,6 +165,7 @@ GKOB_V(float, f32)
         static constexpr auto csr_advanced_spmv = b200_csr_advanced_spmv_##S##_##T;             \
         static constexpr auto csr_spmv_dot = b200_csr_spmv_dot_##S##_##T;                       \
         static constexpr auto csr_spmv_dot2 = b200_csr_spmv_dot2_##S##_##T;                     \
+        static constexpr auto csr_spmv_sub_dot = b200_csr_spmv_sub_dot_##S##_##T;               \
         static constexpr auto csr_spmv_mdot = b200_csr_spmv_mdot_##S##_##T;                     \
         static constexpr auto csr_spmv_mdot2 = b200_csr_spmv_mdot2_##S##_##T;                   \
         static constexpr auto csr_extract_diagonal = b200_csr_extract_diagonal_##S##_##T;       \

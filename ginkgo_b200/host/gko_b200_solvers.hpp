@@ -1541,6 +1541,20 @@ class Minres : public SolverBase<V> {
 
 public:
     struct Factory : SolverFactoryBase<Factory> {
+        bool fused_ = false;
+        int check_every_ = 16;
+        // ginkgo_b200 extension: device-resident fused iteration where applicable (default off)
+        Factory& with_fused(bool f)
+        {
+            fused_ = f;
+            return *this;
+        }
+        // iterations per graph launch (and per read of the control block) on the fused path
+        Factory& with_check_every(int k)
+        {
+            check_every_ = k;
+            return *this;
+        }
         std::unique_ptr<LinOp> generate(std::shared_ptr<const LinOp> op) const override
         {
             auto exec = this->exec_ ? this->exec_ : op->get_executor();
@@ -1548,16 +1562,21 @@ public:
         }
     };
     static Factory build() { return Factory{}; }
+    bool used_fused_path() const { return used_fused_; }
+    ~Minres() override { b200_graph_destroy(graph_); }
 
 protected:
     Minres(std::shared_ptr<const Executor> exec, const Factory& f, std::shared_ptr<const LinOp> op)
-        : Base(exec, f, op)
+        : Base(exec, f, op), fused_(f.fused_), check_every_(std::max(1, f.check_every_))
     {}
     using Base::apply_impl;
     void apply_impl(const LinOp* lb, LinOp* lx) const override
     {
         auto b = as<Dense>(lb);
         auto x = as<Dense>(lx);
+        if (fused_ && try_fused<int32>(b, x)) return;
+        if (fused_ && try_fused<int64>(b, x)) return;
+        used_fused_ = false;
         auto exec = this->exec_;
         auto ctx = exec->ctx();
         const dim2 sz = b->get_size();
@@ -1609,6 +1628,100 @@ protected:
         }
         this->record(iter, stop_status);
     }
+
+    // Fused device-resident path (csrc/fused_minres.cu): three launches per iteration, a graph of
+    // check_every iterations per read of the control block.  The set-up is the loop's own calls.
+    // ResidualNorm recomputes b - A x from the solution at every check, so it keeps the loop.
+    template <typename I>
+    bool try_fused(const Dense* b, Dense* x) const
+    {
+        typename Base::template FusedProblem<I> f;
+        if (!this->template fused_problem<I>(b, x, f) || !this->template fused_scalar_preconditioner<I>(f) ||
+            f.res_kind == 1)
+            return false;
+        const auto A = f.A;
+        const V* inv_diag = f.inv_diag;
+        auto exec = this->exec_;
+        auto ctx = exec->ctx();
+        const int64 n = this->size_.rows;
+        const int64 nnz = A->get_num_stored_elements();
+        // workspace (kept across applies: pointers are baked into the iteration graph)
+        if (!ws_ || ws_n_ != n) {
+            ws_ = Dense::create(exec, dim2{(size_type)(6 * n), 1});
+            sc_ = array<V>(exec, 16);
+            ctl_ = array<int32>(exec, 8);
+            stop_ = array<uint8>(exec, 1);
+            work_ = array<V>(exec, (size_type)vabi<V>::minres_fused_work_size(ctx));
+            ws_n_ = n;
+            b200_graph_destroy(graph_);
+            graph_ = nullptr;
+        }
+        V* r = ws_->get_values();
+        V *z = r + n, *q = r + 2 * n, *v = r + 3 * n, *p0 = r + 4 * n, *p1 = r + 5 * n;
+        V* xv = x->get_values();
+        V* sc = sc_.get_data();
+        int32* ctl = ctl_.get_data();
+        auto view = [&](V* d, int64 rows) { return Dense::create_view(exec, dim2{(size_type)rows, 1}, d, 1); };
+        auto rv = view(r, n), zv = view(z, n);
+        // the loop's set-up: r = b - A x, z = M r, beta = r.z, tau = z.z, minres::initialize (q_prev
+        // is not kept: its zeros go to v, which initialize zeroes as well)
+        exec->copy(r, b->get_const_values(), n);
+        A->apply(this->neg_one_.get(), x, this->one_.get(), rv.get());
+        this->preconditioner_->apply(rv.get(), zv.get());
+        rv->compute_conj_dot(zv.get(), view(sc + 1, 1).get());
+        zv->compute_conj_dot(zv.get(), view(sc + 6, 1).get());
+        GKOB_CALL(vabi<V>::minres_initialize(ctx, n, 1, r, 1, z, 1, p0, 1, p1, 1, q, 1, v, 1, v, 1, sc + 1,
+                                             sc + 2, sc + 3, sc + 9, sc + 10, sc + 11, sc + 12, sc + 8, sc + 7,
+                                             stop_.get_data()));
+        if (f.baseline == 0) b->compute_norm2(view(sc + 4, 1).get());
+        if (f.baseline == 1) rv->compute_norm2(view(sc + 4, 1).get());
+        GKOB_CALL(vabi<V>::minres_fused_init(ctx, sc, ctl, f.max_iters, f.res_kind, f.iter_first, f.baseline,
+                                             (V)f.factor));
+        auto enqueue_iteration = [&]() {
+            GKOB_CALL((viabi<V, I>::csr_spmv_sub_dot(ctx, A->get_plan(), n, n, nnz, A->get_const_row_ptrs(),
+                                                     A->get_const_col_idxs(), A->get_const_values(), z, v, sc,
+                                                     work_.get_data(), ctl)));
+            GKOB_CALL(vabi<V>::minres_fused_lanczos(ctx, n, v, q, inv_diag, sc, ctl, work_.get_data()));
+            GKOB_CALL(vabi<V>::minres_fused_update(ctx, n, xv, p0, p1, z, q, v, inv_diag, sc, ctl));
+        };
+        const MultiRhsKey key{1, r, xv, inv_diag, A->get_const_row_ptrs(), A->get_const_col_idxs(),
+                              A->get_const_values(), nnz};
+        if (!graph_ || !(graph_key_ == key)) {
+            b200_graph_destroy(graph_);
+            graph_ = nullptr;
+            (void)A->get_plan();  // not inside the capture
+            GKOB_CALL(b200_graph_begin_capture(ctx));
+            for (int k = 0; k < check_every_; ++k) enqueue_iteration();
+            GKOB_CALL(b200_graph_end_capture(ctx, &graph_));
+            graph_key_ = key;
+        }
+        int32 h[8] = {0};
+        exec->copy_to_host(h, ctl_.get_const_data(), 8);
+        while (h[0] == 0) {
+            const int32 before = h[1];
+            GKOB_CALL(b200_graph_launch(ctx, graph_));
+            exec->copy_to_host(h, ctl_.get_const_data(), 8);
+            if (h[0] == 0 && h[1] == before)
+                throw Error("fused MINRES: the device iteration made no progress");
+        }
+        this->num_iterations_ = (size_type)h[1];
+        this->status_.assign(1, (uint8)h[0]);
+        used_fused_ = true;
+        return true;
+    }
+
+private:
+    using MultiRhsKey = typename Base::MultiRhsKey;
+    bool fused_;
+    int check_every_;
+    mutable bool used_fused_ = false;
+    mutable std::unique_ptr<Dense> ws_;
+    mutable array<V> sc_, work_;
+    mutable array<int32> ctl_;
+    mutable array<uint8> stop_;
+    mutable int64 ws_n_ = -1;
+    mutable b200_graph* graph_ = nullptr;
+    mutable MultiRhsKey graph_key_;
 };
 
 // ---------------------------------------------------------------------------------------------

@@ -705,6 +705,62 @@ B200_DECL_SPMV_DOT2(f32, float, i32, int32_t)
 B200_DECL_SPMV_DOT2(f32, float, i64, int64_t)
 
 /* ---------------------------------------------------------------------------
+ * Fused MINRES iteration (ginkgo_b200 extension behind solver::Minres::apply with with_fused(true),
+ * single GPU; it regroups the loop body of core/solver/minres.cpp:199-285 into three launches per
+ * iteration with every scalar produced and consumed on the device; d = inv_diag of a scalar
+ * Jacobi preconditioner, NULL for Identity):
+ *   spmv_sub_dot  v = A z - v, alpha = z.v in the SpMV epilogue
+ *                                                   (Csr::apply(1, z, -1, v) + compute_conj_dot)
+ *   lanczos       v -= alpha q (not when alpha == 0); beta = v.(d v); then in the last CTA
+ *                 minres::step_1: beta = sqrt(beta), the two old rotations, the new Givens
+ *                 rotation, tau, eta and eta_next   (sub_scaled + jacobi apply + compute_conj_dot
+ *                                                    + minres::step_1)
+ *   update        minres::step_2 with z~ = d v recomputed and q_prev not stored: p = (z - gamma
+ *                 p_prev - delta p) / alpha; x += cos eta p; q = v / beta; v = q_old beta;
+ *                 z = z~ / beta (0 for a zero divisor).  p / p_prev are p0 / p1 as the parity of
+ *                 the iteration count says (iteration k writes p1 when k is even, p0 when odd).
+ *                 The last CTA swaps gamma / beta, counts the iteration and runs the criterion
+ *                 check of the next one       (std::swap(p, p_prev) + minres::step_2 + std::swap
+ *                                              (gamma, beta) + criterion check)
+ *   init          the first criterion check, after the host's minres::initialize; sc[4] holds
+ *                 ||b|| (baseline 0) or ||r0|| (1) and is set to 1 for baseline 2
+ * sc:  VT[16]   0 alpha, 1 beta, 2 gamma, 3 delta, 4 tau0, 5 threshold, 6 tau, 7 eta, 8 eta_next,
+ *               9 cos_prev, 10 cos, 11 sin_prev, 12 sin
+ * ctl: int32[8] 0 stopping_status byte (0 = running), 1 iterations, 2 max_iters (-1 none),
+ *               3 res_kind (0 none, 2 ImplicitResidualNorm: sqrt|tau| <= threshold), 4 iter_first
+ * With ctl[0] != 0 every kernel is a no-op, so graphs of k iterations can be replayed and the host
+ * polls ctl every k iterations.  `work` has b200_minres_fused_work_size elements.
+ *
+ * b200_csr_spmv_sub_dot: c = A b - c and *dot_out = b . c in one launch (square A): the advanced
+ * SpMV with alpha = 1, beta = -1, bit for bit b200_csr_advanced_spmv on a plan without column
+ * parts.  Plan, work, ctl and alignment rules are those of b200_csr_spmv_dot.
+ * ------------------------------------------------------------------------- */
+#define B200_DECL_FMINRES(V, VT)                                                               \
+    int64_t b200_minres_fused_work_size_##V(const b200_ctx* ctx);                              \
+    b200_status b200_minres_fused_init_##V(b200_ctx* ctx, VT* sc, int32_t* ctl,                \
+                                           int64_t max_iters, int32_t res_kind,                \
+                                           int32_t iter_first, int32_t baseline,               \
+                                           VT reduction_factor);                               \
+    b200_status b200_minres_fused_lanczos_##V(b200_ctx* ctx, int64_t n, VT* v, const VT* q,    \
+                                              const VT* inv_diag, VT* sc, const int32_t* ctl,  \
+                                              VT* work);                                       \
+    b200_status b200_minres_fused_update_##V(b200_ctx* ctx, int64_t n, VT* x, VT* p0, VT* p1,  \
+                                             VT* z, VT* q, VT* v, const VT* inv_diag, VT* sc,  \
+                                             int32_t* ctl);
+#define B200_DECL_SPMV_SUB_DOT(V, VT, I, IT)                                                   \
+    b200_status b200_csr_spmv_sub_dot_##V##_##I(                                               \
+        b200_ctx* ctx, const b200_csr_plan* plan, int64_t num_rows, int64_t num_cols,          \
+        int64_t nnz, const IT* row_ptrs, const IT* col_idxs, const VT* values, const VT* b,    \
+        VT* c, VT* dot_out, VT* work, const int32_t* ctl);
+
+B200_DECL_FMINRES(f64, double)
+B200_DECL_FMINRES(f32, float)
+B200_DECL_SPMV_SUB_DOT(f64, double, i32, int32_t)
+B200_DECL_SPMV_SUB_DOT(f64, double, i64, int64_t)
+B200_DECL_SPMV_SUB_DOT(f32, float, i32, int32_t)
+B200_DECL_SPMV_SUB_DOT(f32, float, i64, int64_t)
+
+/* ---------------------------------------------------------------------------
  * Fused CG iteration for k = 2..32 right-hand sides (ginkgo_b200 extension behind solver::Cg::apply
  * with with_fused_multi_rhs(true), single GPU).  The regrouping of the fused CG above with every
  * vector n x k row-major (stride k) and every scalar per column; one matrix pass per iteration
