@@ -664,7 +664,7 @@ protected:
         num_iterations_ = iters;
         status_ = stop.to_host();
     }
-    // What the fused device-resident iterations (Cg, Bicgstab, Gmres) take: a Csr matrix with
+    // What the fused device-resident iterations (Cg, Bicgstab, Gmres, Minres) take: a Csr matrix with
     // 16-byte-aligned arrays, 1..max_cols right-hand sides stored without gaps (stride == columns)
     // and no reducer (rows of a distributed vector take the loop with its all-reduces), and one or
     // two criteria out of Iteration / (Implicit)ResidualNorm.  Which preconditioners each takes is
@@ -717,31 +717,90 @@ protected:
         }
         return !((((std::uintptr_t)f.A->get_const_col_idxs()) | ((std::uintptr_t)f.A->get_const_values())) & 15);
     }
-    // the several-column fused paths of Cg and Bicgstab keep their workspace, control block and graph
-    // across applies; what the graph bakes in (the index arrays as untyped pointers: int32 or int64)
-    struct MultiRhsKey {
-        int64 k = 0;
+    // What a fused path's graphs bake in besides their launch sequence.  Each path fills in what its
+    // own graphs hold and leaves the rest null.  pre is the preconditioner's storage: the Jacobi blocks
+    // (the inverted diagonal when scalar), their precisions and block pointers.  The index arrays are
+    // untyped pointers (int32 or int64).
+    struct FusedKey {
+        int64 k = 0, nnz = -1;
         const V* ws = nullptr;
         const V* x = nullptr;
-        const V* inv_diag = nullptr;
+        const void* pre[3] = {};
         const void* row_ptrs = nullptr;
         const void* col_idxs = nullptr;
         const V* values = nullptr;
-        int64 nnz = -1;
-        bool operator==(const MultiRhsKey& o) const
+        const void* plan = nullptr;
+        bool operator==(const FusedKey& o) const
         {
-            return k == o.k && ws == o.ws && x == o.x && inv_diag == o.inv_diag && row_ptrs == o.row_ptrs &&
-                   col_idxs == o.col_idxs && values == o.values && nnz == o.nnz;
+            return k == o.k && nnz == o.nnz && ws == o.ws && x == o.x && std::equal(pre, pre + 3, o.pre) &&
+                   row_ptrs == o.row_ptrs && col_idxs == o.col_idxs && values == o.values && plan == o.plan;
         }
     };
-    struct MultiRhsState {
+    // A fused path's workspace, control block and graphs, kept across applies: the graphs bake in the
+    // workspace's pointers
+    struct FusedState {
         std::unique_ptr<Dense> ws;
         array<V> sc, work;
         array<uint8> status;
         array<int32> ctl;
         int64 n = -1, k = 0;
-        b200_graph* graph = nullptr;
-        MultiRhsKey key;
+        std::vector<b200_graph*> graphs;
+        FusedKey key;
+        ~FusedState() { drop(); }
+        void drop()
+        {
+            for (auto g : graphs) b200_graph_destroy(g);
+            graphs.clear();
+            key = FusedKey{};
+        }
+        // alloc() (re)allocates the workspace for n rows and k columns when either changed; the graphs
+        // hold the pointers it frees
+        template <typename Alloc>
+        void reshape(int64 rows, int64 cols, Alloc alloc)
+        {
+            if (n == rows && k == cols) return;
+            drop();
+            alloc();
+            n = rows;
+            k = cols;
+        }
+        // Unless the cached graphs were captured for this key, capture `batches` new ones; enqueue(i)
+        // enqueues batch i.  Whatever the capture bakes in must exist before it: a Csr's plan comes from
+        // get_plan() before, never inside, begin_capture.
+        template <typename Enqueue>
+        void capture(b200_ctx* ctx, const FusedKey& new_key, int64 batches, Enqueue enqueue)
+        {
+            if (!graphs.empty() && key == new_key) return;
+            drop();
+            for (int64 i = 0; i < batches; ++i) {
+                b200_graph* g = nullptr;
+                GKOB_CALL(b200_graph_begin_capture(ctx));
+                enqueue(i);
+                GKOB_CALL(b200_graph_end_capture(ctx, &g));
+                graphs.push_back(g);
+            }
+            key = new_key;
+        }
+        // One GPU: launch the graph next() names (next() also does the host work between batches), read
+        // the control block, launch the next, until ctl[0] is set; returns (ctl[0], ctl[1]), the stop
+        // flags and the iteration count.  (The distributed solver keeps a batch queued ahead through
+        // b200_snapshot_* because there every rank's GPU waits for the slowest HOST; on one GPU the two
+        // loops measure the same -- 3400 vs 3394 it/s on cfg3 -- so the simple one stays.)
+        template <typename Next>
+        std::pair<int32, int32> poll(const Executor& exec, const char* path, Next next) const
+        {
+            int32 h[8] = {0};
+            exec.copy_to_host(h, ctl.get_const_data(), 8);
+            while (h[0] == 0) {
+                const size_type g = next();
+                const int32 before = h[1];
+                GKOB_CALL(b200_graph_launch(exec.ctx(), graphs[g]));
+                exec.copy_to_host(h, ctl.get_const_data(), 8);
+                if (h[0] == 0 && h[1] == before)
+                    throw Error(std::string(path) + ": the device iteration made no progress");
+            }
+            return {h[0], h[1]};
+        }
     };
     std::shared_ptr<const LinOp> system_matrix_;
     std::shared_ptr<const LinOp> preconditioner_;
@@ -850,11 +909,6 @@ public:
     };
     static Factory build() { return Factory{}; }
     bool used_fused_path() const { return used_fused_; }
-    ~Cg() override
-    {
-        b200_graph_destroy(graph_);
-        b200_graph_destroy(mrhs_.graph);
-    }
 
 protected:
     Cg(std::shared_ptr<const Executor> exec, const Factory& f, std::shared_ptr<const LinOp> op)
@@ -939,64 +993,43 @@ protected:
         auto ctx = exec->ctx();
         const int64 n = this->size_.rows;
         const int64 nnz = A->get_num_stored_elements();
-        // workspace (kept across applies: pointers are baked into the iteration graph)
-        if (!ws_ || ws_n_ != n) {
-            ws_ = Dense::create(exec, dim2{(size_type)(4 * n), 1});
-            sc_ = array<V>(exec, 8);
-            ctl_ = array<int32>(exec, 8);
-            work_ = array<V>(exec, (size_type)vabi<V>::fused_work_size(ctx));
-            ws_n_ = n;
-            b200_graph_destroy(graph_);
-            graph_ = nullptr;
-        }
-        V* r = ws_->get_values();
+        auto& s = single_;
+        s.reshape(n, 1, [&] {
+            s.ws = Dense::create(exec, dim2{(size_type)(4 * n), 1});
+            s.sc = array<V>(exec, 8);
+            s.ctl = array<int32>(exec, 8);
+            s.work = array<V>(exec, (size_type)vabi<V>::fused_work_size(ctx));
+        });
+        V* r = s.ws->get_values();
         V* z = r + n;
         V* p = z + n;
         V* q = p + n;
         V* xv = x->get_values();
+        V* sc = s.sc.get_data();
+        int32* ctl = s.ctl.get_data();
+        V* work = s.work.get_data();
         // r = b - A x
         exec->copy(r, b->get_const_values(), n);
         auto rview = Dense::create_view(exec, dim2{(size_type)n, 1}, r, 1);
         A->apply(this->neg_one_.get(), x, this->one_.get(), rview.get());
         if (baseline == 0)  // ||b|| into sc[4]
-            GKOB_CALL(vabi<V>::norm2(ctx, n, 1, b->get_const_values(), 1, sc_.get_data() + 4));
-        GKOB_CALL(vabi<V>::fused_init(ctx, n, r, z, p, q, inv_diag, sc_.get_data(), ctl_.get_data(),
-                                      work_.get_data(), max_iters, res_kind, iter_first, baseline,
-                                      (V)factor, 1));
-        auto enqueue_iteration = [&]() {
-            GKOB_CALL(vabi<V>::fused_step_p(ctx, n, p, z, sc_.get_const_data(), ctl_.get_const_data()));
-            GKOB_CALL((viabi<V, I>::csr_spmv_dot(ctx, A->get_plan(), n, n, nnz, A->get_const_row_ptrs(),
-                                                 A->get_const_col_idxs(), A->get_const_values(), p, q,
-                                                 sc_.get_data() + 2, work_.get_data(),
-                                                 ctl_.get_const_data())));
-            GKOB_CALL(vabi<V>::fused_step_xr(ctx, n, xv, r, p, q, z, inv_diag, sc_.get_data(),
-                                             ctl_.get_data(), work_.get_data(), 1));
-        };
-        if (!graph_ || graph_x_ != xv || graph_diag_ != inv_diag) {
-            b200_graph_destroy(graph_);
-            graph_ = nullptr;
-            (void)A->get_plan();  // not inside the capture
-            GKOB_CALL(b200_graph_begin_capture(ctx));
-            for (int k = 0; k < check_every_; ++k) enqueue_iteration();
-            GKOB_CALL(b200_graph_end_capture(ctx, &graph_));
-            graph_x_ = xv;
-            graph_diag_ = inv_diag;
-        }
-        // One GPU: launch a batch, read the control block, launch the next.  (The distributed solver
-        // keeps a batch queued ahead through b200_snapshot_* because there every rank's GPU waits for
-        // the slowest HOST; on one GPU the two loops measure the same -- 3400 vs 3394 it/s on cfg3 --
-        // so the simple one stays.)
-        int32 h[8] = {0};
-        exec->copy_to_host(h, ctl_.get_const_data(), 8);
-        while (h[0] == 0) {
-            const int32 before = h[1];
-            GKOB_CALL(b200_graph_launch(ctx, graph_));
-            exec->copy_to_host(h, ctl_.get_const_data(), 8);
-            if (h[0] == 0 && h[1] == before)
-                throw Error("fused CG: the device iteration made no progress");
-        }
-        this->num_iterations_ = (size_type)h[1];
-        this->status_.assign(1, (uint8)h[0]);
+            GKOB_CALL(vabi<V>::norm2(ctx, n, 1, b->get_const_values(), 1, sc + 4));
+        GKOB_CALL(vabi<V>::fused_init(ctx, n, r, z, p, q, inv_diag, sc, ctl, work, max_iters, res_kind,
+                                      iter_first, baseline, (V)factor, 1));
+        const FusedKey key{1, nnz, r, xv, {inv_diag}, A->get_const_row_ptrs(), A->get_const_col_idxs(),
+                           A->get_const_values(), A->get_plan()};
+        s.capture(ctx, key, 1, [&](int64) {
+            for (int k = 0; k < check_every_; ++k) {
+                GKOB_CALL(vabi<V>::fused_step_p(ctx, n, p, z, sc, ctl));
+                GKOB_CALL((viabi<V, I>::csr_spmv_dot(ctx, A->get_plan(), n, n, nnz, A->get_const_row_ptrs(),
+                                                     A->get_const_col_idxs(), A->get_const_values(), p, q,
+                                                     sc + 2, work, ctl)));
+                GKOB_CALL(vabi<V>::fused_step_xr(ctx, n, xv, r, p, q, z, inv_diag, sc, ctl, work, 1));
+            }
+        });
+        const auto [flags, iters] = s.poll(*exec, "fused CG", [] { return 0; });
+        this->num_iterations_ = (size_type)iters;
+        this->status_.assign(1, (uint8)flags);
         used_fused_ = true;
         return true;
     }
@@ -1019,19 +1052,14 @@ protected:
         const int64 k = (int64)b->get_size().cols;
         const int64 nnz = A->get_num_stored_elements();
         auto& m = mrhs_;
-        // workspace r, z, p, q (n x k each), per-column scalars, statuses, control block, partials;
-        // kept across applies
-        if (!m.ws || m.n != n || m.k != k) {
+        // workspace r, z, p, q (n x k each), per-column scalars, statuses, control block, partials
+        m.reshape(n, k, [&] {
             m.ws = Dense::create(exec, dim2{(size_type)(4 * n * k), 1});
             m.sc = array<V>(exec, (size_type)(6 * k));
             m.status = array<uint8>(exec, (size_type)k);
             m.ctl = array<int32>(exec, 8);
             m.work = array<V>(exec, (size_type)vabi<V>::cg_mrhs_work_size(ctx, k));
-            m.n = n;
-            m.k = k;
-            b200_graph_destroy(m.graph);  // it holds the pointers just freed
-            m.graph = nullptr;
-        }
+        });
         V* r = m.ws->get_values();
         V* z = r + n * k;
         V* p = z + n * k;
@@ -1047,13 +1075,9 @@ protected:
         GKOB_CALL(vabi<V>::cg_mrhs_init(ctx, n, k, r, z, p, q, f.inv_diag, sc, m.status.get_data(),
                                         m.ctl.get_data(), m.work.get_data(), f.max_iters, f.res_kind,
                                         f.iter_first, f.baseline, (V)f.factor));
-        // the graph bakes in every pointer and size below: re-capture when one changes
-        const MultiRhsKey key{k, r, xv, f.inv_diag, A->get_const_row_ptrs(), A->get_const_col_idxs(),
-                              A->get_const_values(), nnz};
-        if (!m.graph || !(m.key == key)) {
-            b200_graph_destroy(m.graph);
-            m.graph = nullptr;
-            GKOB_CALL(b200_graph_begin_capture(ctx));
+        const FusedKey key{k, nnz, r, xv, {f.inv_diag}, A->get_const_row_ptrs(), A->get_const_col_idxs(),
+                           A->get_const_values()};
+        m.capture(ctx, key, 1, [&](int64) {
             for (int it = 0; it < check_every_; ++it) {
                 GKOB_CALL(vabi<V>::cg_mrhs_step_p(ctx, n, k, p, z, sc, m.status.get_const_data(),
                                                   m.ctl.get_const_data()));
@@ -1065,20 +1089,8 @@ protected:
                                                    m.status.get_data(), m.ctl.get_data(),
                                                    m.work.get_data()));
             }
-            GKOB_CALL(b200_graph_end_capture(ctx, &m.graph));
-            m.key = key;
-        }
-        int32 h[8] = {0};
-        exec->copy_to_host(h, m.ctl.get_const_data(), 8);
-        while (h[0] == 0) {
-            const int32 before = h[1];
-            GKOB_CALL(b200_graph_launch(ctx, m.graph));
-            exec->copy_to_host(h, m.ctl.get_const_data(), 8);
-            if (h[0] == 0 && h[1] == before)
-                throw Error("fused CG (several right-hand sides): the device iteration made no progress");
-        }
-        this->num_iterations_ = (size_type)h[1];
-        this->status_ = m.status.to_host();
+        });
+        this->record(m.poll(*exec, "fused CG (several right-hand sides)", [] { return 0; }).second, m.status);
         used_fused_ = true;
         return true;
     }
@@ -1088,15 +1100,8 @@ private:
     bool fused_multi_rhs_;
     int check_every_;
     mutable bool used_fused_ = false;
-    mutable std::unique_ptr<Dense> ws_;
-    mutable array<V> sc_, work_;
-    mutable array<int32> ctl_;
-    mutable int64 ws_n_ = -1;
-    mutable b200_graph* graph_ = nullptr;
-    mutable const V* graph_x_ = nullptr;
-    mutable const V* graph_diag_ = nullptr;
-    using MultiRhsKey = typename Base::MultiRhsKey;
-    mutable typename Base::MultiRhsState mrhs_;
+    using FusedKey = typename Base::FusedKey;
+    mutable typename Base::FusedState single_, mrhs_;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -1563,7 +1568,6 @@ public:
     };
     static Factory build() { return Factory{}; }
     bool used_fused_path() const { return used_fused_; }
-    ~Minres() override { b200_graph_destroy(graph_); }
 
 protected:
     Minres(std::shared_ptr<const Executor> exec, const Factory& f, std::shared_ptr<const LinOp> op)
@@ -1645,22 +1649,20 @@ protected:
         auto ctx = exec->ctx();
         const int64 n = this->size_.rows;
         const int64 nnz = A->get_num_stored_elements();
-        // workspace (kept across applies: pointers are baked into the iteration graph)
-        if (!ws_ || ws_n_ != n) {
-            ws_ = Dense::create(exec, dim2{(size_type)(6 * n), 1});
-            sc_ = array<V>(exec, 16);
-            ctl_ = array<int32>(exec, 8);
-            stop_ = array<uint8>(exec, 1);
-            work_ = array<V>(exec, (size_type)vabi<V>::minres_fused_work_size(ctx));
-            ws_n_ = n;
-            b200_graph_destroy(graph_);
-            graph_ = nullptr;
-        }
-        V* r = ws_->get_values();
+        auto& s = single_;
+        s.reshape(n, 1, [&] {
+            s.ws = Dense::create(exec, dim2{(size_type)(6 * n), 1});
+            s.sc = array<V>(exec, 16);
+            s.ctl = array<int32>(exec, 8);
+            s.status = array<uint8>(exec, 1);
+            s.work = array<V>(exec, (size_type)vabi<V>::minres_fused_work_size(ctx));
+        });
+        V* r = s.ws->get_values();
         V *z = r + n, *q = r + 2 * n, *v = r + 3 * n, *p0 = r + 4 * n, *p1 = r + 5 * n;
         V* xv = x->get_values();
-        V* sc = sc_.get_data();
-        int32* ctl = ctl_.get_data();
+        V* sc = s.sc.get_data();
+        int32* ctl = s.ctl.get_data();
+        V* work = s.work.get_data();
         auto view = [&](V* d, int64 rows) { return Dense::create_view(exec, dim2{(size_type)rows, 1}, d, 1); };
         auto rv = view(r, n), zv = view(z, n);
         // the loop's set-up: r = b - A x, z = M r, beta = r.z, tau = z.z, minres::initialize (q_prev
@@ -1672,56 +1674,35 @@ protected:
         zv->compute_conj_dot(zv.get(), view(sc + 6, 1).get());
         GKOB_CALL(vabi<V>::minres_initialize(ctx, n, 1, r, 1, z, 1, p0, 1, p1, 1, q, 1, v, 1, v, 1, sc + 1,
                                              sc + 2, sc + 3, sc + 9, sc + 10, sc + 11, sc + 12, sc + 8, sc + 7,
-                                             stop_.get_data()));
+                                             s.status.get_data()));
         if (f.baseline == 0) b->compute_norm2(view(sc + 4, 1).get());
         if (f.baseline == 1) rv->compute_norm2(view(sc + 4, 1).get());
         GKOB_CALL(vabi<V>::minres_fused_init(ctx, sc, ctl, f.max_iters, f.res_kind, f.iter_first, f.baseline,
                                              (V)f.factor));
-        auto enqueue_iteration = [&]() {
-            GKOB_CALL((viabi<V, I>::csr_spmv_sub_dot(ctx, A->get_plan(), n, n, nnz, A->get_const_row_ptrs(),
-                                                     A->get_const_col_idxs(), A->get_const_values(), z, v, sc,
-                                                     work_.get_data(), ctl)));
-            GKOB_CALL(vabi<V>::minres_fused_lanczos(ctx, n, v, q, inv_diag, sc, ctl, work_.get_data()));
-            GKOB_CALL(vabi<V>::minres_fused_update(ctx, n, xv, p0, p1, z, q, v, inv_diag, sc, ctl));
-        };
-        const MultiRhsKey key{1, r, xv, inv_diag, A->get_const_row_ptrs(), A->get_const_col_idxs(),
-                              A->get_const_values(), nnz};
-        if (!graph_ || !(graph_key_ == key)) {
-            b200_graph_destroy(graph_);
-            graph_ = nullptr;
-            (void)A->get_plan();  // not inside the capture
-            GKOB_CALL(b200_graph_begin_capture(ctx));
-            for (int k = 0; k < check_every_; ++k) enqueue_iteration();
-            GKOB_CALL(b200_graph_end_capture(ctx, &graph_));
-            graph_key_ = key;
-        }
-        int32 h[8] = {0};
-        exec->copy_to_host(h, ctl_.get_const_data(), 8);
-        while (h[0] == 0) {
-            const int32 before = h[1];
-            GKOB_CALL(b200_graph_launch(ctx, graph_));
-            exec->copy_to_host(h, ctl_.get_const_data(), 8);
-            if (h[0] == 0 && h[1] == before)
-                throw Error("fused MINRES: the device iteration made no progress");
-        }
-        this->num_iterations_ = (size_type)h[1];
-        this->status_.assign(1, (uint8)h[0]);
+        const FusedKey key{1, nnz, r, xv, {inv_diag}, A->get_const_row_ptrs(), A->get_const_col_idxs(),
+                           A->get_const_values(), A->get_plan()};
+        s.capture(ctx, key, 1, [&](int64) {
+            for (int k = 0; k < check_every_; ++k) {
+                GKOB_CALL((viabi<V, I>::csr_spmv_sub_dot(ctx, A->get_plan(), n, n, nnz, A->get_const_row_ptrs(),
+                                                         A->get_const_col_idxs(), A->get_const_values(), z, v, sc,
+                                                         work, ctl)));
+                GKOB_CALL(vabi<V>::minres_fused_lanczos(ctx, n, v, q, inv_diag, sc, ctl, work));
+                GKOB_CALL(vabi<V>::minres_fused_update(ctx, n, xv, p0, p1, z, q, v, inv_diag, sc, ctl));
+            }
+        });
+        const auto [flags, iters] = s.poll(*exec, "fused MINRES", [] { return 0; });
+        this->num_iterations_ = (size_type)iters;
+        this->status_.assign(1, (uint8)flags);
         used_fused_ = true;
         return true;
     }
 
 private:
-    using MultiRhsKey = typename Base::MultiRhsKey;
+    using FusedKey = typename Base::FusedKey;
     bool fused_;
     int check_every_;
     mutable bool used_fused_ = false;
-    mutable std::unique_ptr<Dense> ws_;
-    mutable array<V> sc_, work_;
-    mutable array<int32> ctl_;
-    mutable array<uint8> stop_;
-    mutable int64 ws_n_ = -1;
-    mutable b200_graph* graph_ = nullptr;
-    mutable MultiRhsKey graph_key_;
+    mutable typename Base::FusedState single_;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -1938,11 +1919,6 @@ public:
     };
     static Factory build() { return Factory{}; }
     bool used_fused_path() const { return used_fused_; }
-    ~Bicgstab() override
-    {
-        b200_graph_destroy(graph_);
-        b200_graph_destroy(mrhs_.graph);
-    }
 
 protected:
     Bicgstab(std::shared_ptr<const Executor> exec, const Factory& f, std::shared_ptr<const LinOp> op)
@@ -2039,65 +2015,48 @@ protected:
         auto ctx = exec->ctx();
         const int64 n = this->size_.rows;
         const int64 nnz = A->get_num_stored_elements();
-        // workspace (kept across applies: pointers are baked into the iteration graph)
-        if (!ws_ || ws_n_ != n) {
-            ws_ = Dense::create(exec, dim2{(size_type)(8 * n), 1});
-            sc_ = array<V>(exec, 16);
-            ctl_ = array<int32>(exec, 8);
-            work_ = array<V>(exec, (size_type)vabi<V>::fused_work_size(ctx));
-            ws_n_ = n;
-            b200_graph_destroy(graph_);
-            graph_ = nullptr;
-        }
-        V* r = ws_->get_values();
+        auto& st = single_;
+        st.reshape(n, 1, [&] {
+            st.ws = Dense::create(exec, dim2{(size_type)(8 * n), 1});
+            st.sc = array<V>(exec, 16);
+            st.ctl = array<int32>(exec, 8);
+            st.work = array<V>(exec, (size_type)vabi<V>::fused_work_size(ctx));
+        });
+        V* r = st.ws->get_values();
         V *rr = r + n, *p = r + 2 * n, *v = r + 3 * n, *y = r + 4 * n, *s = r + 5 * n, *t = r + 6 * n,
           *z = r + 7 * n;
         V* xv = x->get_values();
-        V* sc = sc_.get_data();
-        int32* ctl = ctl_.get_data();
+        V* sc = st.sc.get_data();
+        int32* ctl = st.ctl.get_data();
+        V* work = st.work.get_data();
         // r = b - A x
         exec->copy(r, b->get_const_values(), n);
         auto rview = Dense::create_view(exec, dim2{(size_type)n, 1}, r, 1);
         A->apply(this->neg_one_.get(), x, this->one_.get(), rview.get());
         if (f.baseline == 0)  // ||b|| into sc[4]
             GKOB_CALL(vabi<V>::norm2(ctx, n, 1, b->get_const_values(), 1, sc + 4));
-        GKOB_CALL(vabi<V>::bicgstab_fused_init(ctx, n, r, rr, p, v, y, s, t, z, sc, ctl, work_.get_data(),
-                                               f.max_iters, f.res_kind, f.iter_first, f.baseline,
-                                               (V)f.factor));
+        GKOB_CALL(vabi<V>::bicgstab_fused_init(ctx, n, r, rr, p, v, y, s, t, z, sc, ctl, work, f.max_iters,
+                                               f.res_kind, f.iter_first, f.baseline, (V)f.factor));
         auto spmv_dot2 = [&](const V* in, V* out, const V* w, V* dot, V* dot2) {
             GKOB_CALL((viabi<V, I>::csr_spmv_dot2(ctx, A->get_plan(), n, n, nnz, A->get_const_row_ptrs(),
                                                   A->get_const_col_idxs(), A->get_const_values(), in, out,
-                                                  w, dot, dot2, work_.get_data(), ctl)));
+                                                  w, dot, dot2, work, ctl)));
         };
-        auto enqueue_iteration = [&]() {
-            GKOB_CALL(vabi<V>::bicgstab_fused_step_p(ctx, n, p, r, v, y, inv_diag, sc, ctl));
-            spmv_dot2(y, v, rr, sc + 2, nullptr);
-            GKOB_CALL(vabi<V>::bicgstab_fused_step_s(ctx, n, r, v, s, z, inv_diag, sc, ctl, work_.get_data()));
-            spmv_dot2(z, t, s, sc + 8, sc + 2);
-            GKOB_CALL(vabi<V>::bicgstab_fused_step_xr(ctx, n, xv, r, s, t, y, z, rr, sc, ctl, work_.get_data()));
-        };
-        if (!graph_ || graph_x_ != xv || graph_diag_ != inv_diag) {
-            b200_graph_destroy(graph_);
-            graph_ = nullptr;
-            (void)A->get_plan();  // not inside the capture
-            GKOB_CALL(b200_graph_begin_capture(ctx));
-            for (int k = 0; k < check_every_; ++k) enqueue_iteration();
-            GKOB_CALL(b200_graph_end_capture(ctx, &graph_));
-            graph_x_ = xv;
-            graph_diag_ = inv_diag;
-        }
+        const FusedKey key{1, nnz, r, xv, {inv_diag}, A->get_const_row_ptrs(), A->get_const_col_idxs(),
+                           A->get_const_values(), A->get_plan()};
+        st.capture(ctx, key, 1, [&](int64) {
+            for (int k = 0; k < check_every_; ++k) {
+                GKOB_CALL(vabi<V>::bicgstab_fused_step_p(ctx, n, p, r, v, y, inv_diag, sc, ctl));
+                spmv_dot2(y, v, rr, sc + 2, nullptr);
+                GKOB_CALL(vabi<V>::bicgstab_fused_step_s(ctx, n, r, v, s, z, inv_diag, sc, ctl, work));
+                spmv_dot2(z, t, s, sc + 8, sc + 2);
+                GKOB_CALL(vabi<V>::bicgstab_fused_step_xr(ctx, n, xv, r, s, t, y, z, rr, sc, ctl, work));
+            }
+        });
         // every captured iteration ends with step_xr, so a stop read here has its finalize applied
-        int32 h[8] = {0};
-        exec->copy_to_host(h, ctl_.get_const_data(), 8);
-        while (h[0] == 0) {
-            const int32 before = h[1];
-            GKOB_CALL(b200_graph_launch(ctx, graph_));
-            exec->copy_to_host(h, ctl_.get_const_data(), 8);
-            if (h[0] == 0 && h[1] == before)
-                throw Error("fused BiCGStab: the device iteration made no progress");
-        }
-        this->num_iterations_ = (size_type)h[1];
-        this->status_.assign(1, (uint8)h[0]);
+        const auto [flags, iters] = st.poll(*exec, "fused BiCGStab", [] { return 0; });
+        this->num_iterations_ = (size_type)iters;
+        this->status_.assign(1, (uint8)flags);
         used_fused_ = true;
         return true;
     }
@@ -2121,18 +2080,14 @@ protected:
         const int64 nnz = A->get_num_stored_elements();
         auto& m = mrhs_;
         // workspace r, rr, p, v, y, s, t, z (n x k each), per-column scalars, statuses, control block,
-        // partials; kept across applies
-        if (!m.ws || m.n != n || m.k != k) {
+        // partials
+        m.reshape(n, k, [&] {
             m.ws = Dense::create(exec, dim2{(size_type)(8 * n * k), 1});
             m.sc = array<V>(exec, (size_type)(10 * k));
             m.status = array<uint8>(exec, (size_type)k);
             m.ctl = array<int32>(exec, 8);
             m.work = array<V>(exec, (size_type)vabi<V>::bicgstab_mrhs_work_size(ctx, k));
-            m.n = n;
-            m.k = k;
-            b200_graph_destroy(m.graph);  // it holds the pointers just freed
-            m.graph = nullptr;
-        }
+        });
         const int64 nk = n * k;
         V* r = m.ws->get_values();
         V *rr = r + nk, *p = r + 2 * nk, *v = r + 3 * nk, *y = r + 4 * nk, *s = r + 5 * nk, *t = r + 6 * nk,
@@ -2156,13 +2111,9 @@ protected:
                                                    A->get_const_values(), in, k, out, w, dots, dots2, work,
                                                    ctl)));
         };
-        // the graph bakes in every pointer and size below: re-capture when one changes
-        const MultiRhsKey key{k, r, xv, inv_diag, A->get_const_row_ptrs(), A->get_const_col_idxs(),
-                              A->get_const_values(), nnz};
-        if (!m.graph || !(m.key == key)) {
-            b200_graph_destroy(m.graph);
-            m.graph = nullptr;
-            GKOB_CALL(b200_graph_begin_capture(ctx));
+        const FusedKey key{k, nnz, r, xv, {inv_diag}, A->get_const_row_ptrs(), A->get_const_col_idxs(),
+                           A->get_const_values()};
+        m.capture(ctx, key, 1, [&](int64) {
             for (int it = 0; it < check_every_; ++it) {
                 GKOB_CALL(vabi<V>::bicgstab_mrhs_step_p(ctx, n, k, p, r, v, y, inv_diag, sc, status, ctl));
                 spmv_mdot2(y, v, rr, sc + 2 * k, nullptr);
@@ -2171,21 +2122,10 @@ protected:
                 GKOB_CALL(vabi<V>::bicgstab_mrhs_step_xr(ctx, n, k, xv, r, s, t, y, z, rr, sc, status, ctl,
                                                          work));
             }
-            GKOB_CALL(b200_graph_end_capture(ctx, &m.graph));
-            m.key = key;
-        }
+        });
         // every captured iteration ends with step_xr, so a stop read here has its finalizes paid
-        int32 h[8] = {0};
-        exec->copy_to_host(h, m.ctl.get_const_data(), 8);
-        while (h[0] == 0) {
-            const int32 before = h[1];
-            GKOB_CALL(b200_graph_launch(ctx, m.graph));
-            exec->copy_to_host(h, m.ctl.get_const_data(), 8);
-            if (h[0] == 0 && h[1] == before)
-                throw Error("fused BiCGStab (several right-hand sides): the device iteration made no progress");
-        }
-        this->num_iterations_ = (size_type)h[1];
-        this->status_ = m.status.to_host();
+        this->record(m.poll(*exec, "fused BiCGStab (several right-hand sides)", [] { return 0; }).second,
+                     m.status);
         used_fused_ = true;
         return true;
     }
@@ -2195,15 +2135,8 @@ private:
     bool fused_multi_rhs_;
     int check_every_;
     mutable bool used_fused_ = false;
-    mutable std::unique_ptr<Dense> ws_;
-    mutable array<V> sc_, work_;
-    mutable array<int32> ctl_;
-    mutable int64 ws_n_ = -1;
-    mutable b200_graph* graph_ = nullptr;
-    mutable const V* graph_x_ = nullptr;
-    mutable const V* graph_diag_ = nullptr;
-    using MultiRhsKey = typename Base::MultiRhsKey;
-    mutable typename Base::MultiRhsState mrhs_;
+    using FusedKey = typename Base::FusedKey;
+    mutable typename Base::FusedState single_, mrhs_;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -2258,11 +2191,6 @@ public:
     };
     static Factory build() { return Factory{}; }
     bool used_fused_path() const { return used_fused_; }
-    ~Gmres() override
-    {
-        drop_graphs();
-        drop_mrhs_graphs();
-    }
 
 protected:
     Gmres(std::shared_ptr<const Executor> exec, const Factory& f, std::shared_ptr<const LinOp> op)
@@ -2444,41 +2372,34 @@ protected:
         auto ctx = exec->ctx();
         const int64 n = this->size_.rows, kd = (int64)krylov_dim_;
         const int64 nnz = A->get_num_stored_elements();
-        // workspace (kept across applies: pointers are baked into the iteration graphs)
-        if (!fkrylov_ || fws_n_ != n) {
+        auto& st = single_;
+        st.reshape(n, 1, [&] {
             fkrylov_ = Dense::create(exec, dim2{(size_type)(n * (kd + 1)), 1});
             fvec_ = Dense::create(exec, dim2{(size_type)(4 * n), 1});  // residual | z | before | after
             fhess_ = Dense::create(exec, dim2{(size_type)kd, (size_type)(kd + 1)});
-            fsmall_ = array<V>(exec, (size_type)(5 * kd + 11));
-            fwork_ = array<V>(exec, (size_type)vabi<V>::gmres_fused_work_size(ctx, kd));
+            st.sc = array<V>(exec, (size_type)(5 * kd + 11));
+            st.work = array<V>(exec, (size_type)vabi<V>::gmres_fused_work_size(ctx, kd));
             ffin_ = array<std::uint64_t>(exec, 1);
-            fstop_ = array<uint8>(exec, 1);
-            fctl_ = array<int32>(exec, 8);
-            fws_n_ = n;
-            drop_graphs();
-        }
-        // what the graphs bake in besides the workspace: the matrix arrays and its SpMV plan, the
-        // preconditioner's storage
-        const void* key[kGraphKey] = {A->get_const_values(), A->get_const_col_idxs(), A->get_const_row_ptrs(),
-                                      A->get_plan(), pre_key[0], pre_key[1], pre_key[2]};
-        if (!std::equal(key, key + kGraphKey, graph_key_)) {
-            drop_graphs();
-            std::copy(key, key + kGraphKey, graph_key_);
-        }
+            st.status = array<uint8>(exec, 1);
+            st.ctl = array<int32>(exec, 8);
+        });
         V* K = fkrylov_->get_values();
+        // x is not baked in: the host's final update applies it
+        const FusedKey key{1, nnz, K, nullptr, {pre_key[0], pre_key[1], pre_key[2]}, A->get_const_row_ptrs(),
+                           A->get_const_col_idxs(), A->get_const_values(), A->get_plan()};
         auto col = [&](int c) {
             return Dense::create_view(exec, dim2{(size_type)n, 1}, fvec_->get_values() + c * n, 1);
         };
         auto residual = col(0), z = col(1), before = col(2), after = col(3);
         V* hess = fhess_->get_values();
         const int64 hs = fhess_->get_stride();
-        V *sc = fsmall_.get_data(), *gsin = sc + 8, *gcos = gsin + kd, *rnc = gcos + kd, *y = rnc + kd + 1,
+        V *sc = st.sc.get_data(), *gsin = sc + 8, *gcos = gsin + kd, *rnc = gcos + kd, *y = rnc + kd + 1,
           *rnorm = y + kd, *haux = rnorm + 1;
         auto rnorm_view = Dense::create_view(exec, dim2{1, 1}, rnorm, 1);
         std::uint64_t* fin = ffin_.get_data();
-        uint8* stop = fstop_.get_data();
-        int32* ctl = fctl_.get_data();
-        V* work = fwork_.get_data();
+        uint8* stop = st.status.get_data();
+        int32* ctl = st.ctl.get_data();
+        V* work = st.work.get_data();
         // the loop's start: fresh Hessenberg, rnc and y; initialize; r = b - A x; ||r||; restart
         fhess_->fill(V(0));
         GKOB_CALL(vabi<V>::fill(ctx, 2 * kd + 1, 1, rnc, 1, V(0)));
@@ -2540,20 +2461,11 @@ protected:
         };
         // batches start at Krylov index 0, c, 2c, ... and end at the restart
         const int64 ce = std::min<int64>(check_every_, kd);
-        if (graphs_.empty()) {
-            (void)A->get_plan();  // not inside the capture
-            for (int64 j0 = 0; j0 < kd; j0 += ce) {
-                b200_graph* g = nullptr;
-                GKOB_CALL(b200_graph_begin_capture(ctx));
-                for (int64 j = j0; j < std::min(j0 + ce, kd); ++j) enqueue_iteration(j);
-                GKOB_CALL(b200_graph_end_capture(ctx, &g));
-                graphs_.push_back(g);
-            }
-        }
-        int32 h[8] = {0};
-        exec->copy_to_host(h, ctl, 8);
+        st.capture(ctx, key, (kd + ce - 1) / ce, [&](int64 i) {
+            for (int64 j = i * ce; j < std::min((i + 1) * ce, kd); ++j) enqueue_iteration(j);
+        });
         int64 j = 0;
-        while (h[0] == 0) {
+        auto next_batch = [&] {
             // the loop's restart, only once the check at the top of iteration krylov_dim said "running"
             if (j == kd) {
                 solve_and_update();
@@ -2563,22 +2475,15 @@ protected:
                 restart();
                 j = 0;
             }
-            const int32 before_iters = h[1];
-            GKOB_CALL(b200_graph_launch(ctx, graphs_[j / ce]));
+            const int64 i = j / ce;
             j = std::min(j + ce, kd);
-            exec->copy_to_host(h, ctl, 8);
-            if (h[0] == 0 && h[1] == before_iters)
-                throw Error("fused GMRES: the device iteration made no progress");
-        }
+            return i;
+        };
+        const int32 iters = st.poll(*exec, "fused GMRES", next_batch).second;
         solve_and_update();
-        this->record((size_type)h[1], fstop_);
+        this->record((size_type)iters, st.status);
         used_fused_ = true;
         return true;
-    }
-    void drop_graphs() const
-    {
-        for (auto g : graphs_) b200_graph_destroy(g);
-        graphs_.clear();
     }
 
     // Fused device-resident path for k = 2..32 right-hand sides (csrc/fused_gmres_mrhs.cu): at Krylov
@@ -2615,8 +2520,8 @@ protected:
         const int64 nnz = A->get_num_stored_elements();
         auto& m = mrhs_;
         // basis n (kd+1) x k; residual, z, before, after n x k each; the Hessenberg kd x (kd+1) k;
-        // sc[3k], gsin, gcos, y (kd x k), rnc, haux ((kd+1) x k), rnorm; kept across applies
-        if (!m.ws || m.n != n || m.k != k) {
+        // sc[3k], gsin, gcos, y (kd x k), rnc, haux ((kd+1) x k), rnorm
+        m.reshape(n, k, [&] {
             m.ws = Dense::create(exec, dim2{(size_type)(nk * (kd + 5)), 1});
             mhess_ = Dense::create(exec, dim2{(size_type)kd, (size_type)((kd + 1) * k)});
             m.sc = array<V>(exec, (size_type)(k * (5 * kd + 6)));
@@ -2624,10 +2529,7 @@ protected:
             m.ctl = array<int32>(exec, 8);
             m.work = array<V>(exec, (size_type)vabi<V>::gmres_mrhs_work_size(ctx, k, kd));
             mfin_ = array<std::uint64_t>(exec, (size_type)k);
-            m.n = n;
-            m.k = k;
-            drop_mrhs_graphs();  // they hold the pointers just freed
-        }
+        });
         V* K = m.ws->get_values();
         auto vec = [&](int c) {
             return Dense::create_view(exec, dim2{(size_type)n, (size_type)k}, K + nk * (kd + 1 + c), (size_type)k);
@@ -2698,26 +2600,16 @@ protected:
             GKOB_CALL(vabi<V>::gmres_mrhs_multi_dot(ctx, n, k, j + 1, kd, K, w, haux, status, ctl, work));
             final_pass(0, haux, haux);
         };
-        // the graphs bake in every pointer and size below: re-capture when one changes.  Batches start at
-        // Krylov index 0, c, 2c, ... and end at the restart.
-        const MultiRhsKey key{k, K, nullptr, inv_diag, A->get_const_row_ptrs(), A->get_const_col_idxs(),
-                              A->get_const_values(), nnz};
+        // x is not baked in: the host's final update applies it.  Batches start at Krylov index 0, c,
+        // 2c, ... and end at the restart.
+        const FusedKey key{k, nnz, K, nullptr, {inv_diag}, A->get_const_row_ptrs(), A->get_const_col_idxs(),
+                           A->get_const_values()};
         const int64 ce = std::min<int64>(check_every_, kd);
-        if (mgraphs_.empty() || !(m.key == key)) {
-            drop_mrhs_graphs();
-            for (int64 j0 = 0; j0 < kd; j0 += ce) {
-                b200_graph* g = nullptr;
-                GKOB_CALL(b200_graph_begin_capture(ctx));
-                for (int64 j = j0; j < std::min(j0 + ce, kd); ++j) enqueue_iteration(j);
-                GKOB_CALL(b200_graph_end_capture(ctx, &g));
-                mgraphs_.push_back(g);
-            }
-            m.key = key;
-        }
-        int32 h[8] = {0};
-        exec->copy_to_host(h, ctl, 8);
+        m.capture(ctx, key, (kd + ce - 1) / ce, [&](int64 i) {
+            for (int64 j = i * ce; j < std::min((i + 1) * ce, kd); ++j) enqueue_iteration(j);
+        });
         int64 j = 0;
-        while (h[0] == 0) {
+        auto next_batch = [&] {
             // the loop's restart on all k columns, only once the check at the top of iteration krylov_dim
             // said "running"
             if (j == kd) {
@@ -2728,22 +2620,15 @@ protected:
                 restart();
                 j = 0;
             }
-            const int32 before_iters = h[1];
-            GKOB_CALL(b200_graph_launch(ctx, mgraphs_[j / ce]));
+            const int64 i = j / ce;
             j = std::min(j + ce, kd);
-            exec->copy_to_host(h, ctl, 8);
-            if (h[0] == 0 && h[1] == before_iters)
-                throw Error("fused GMRES (several right-hand sides): the device iteration made no progress");
-        }
+            return i;
+        };
+        const int32 iters = m.poll(*exec, "fused GMRES (several right-hand sides)", next_batch).second;
         solve_and_update();
-        this->record((size_type)h[1], m.status);
+        this->record((size_type)iters, m.status);
         used_fused_ = true;
         return true;
-    }
-    void drop_mrhs_graphs() const
-    {
-        for (auto g : mgraphs_) b200_graph_destroy(g);
-        mgraphs_.clear();
     }
 
 private:
@@ -2753,21 +2638,15 @@ private:
     bool fused_multi_rhs_;
     int check_every_;
     mutable bool used_fused_ = false;
+    using FusedKey = typename Base::FusedKey;
+    // the one-column path: sc, work, status and ctl in single_, the basis, vectors, Hessenberg and fin here
+    mutable typename Base::FusedState single_;
     mutable std::unique_ptr<Dense> fkrylov_, fvec_, fhess_;
-    mutable array<V> fsmall_, fwork_;
     mutable array<std::uint64_t> ffin_;
-    mutable array<uint8> fstop_;
-    mutable array<int32> fctl_;
-    mutable int64 fws_n_ = -1;
-    mutable std::vector<b200_graph*> graphs_;
-    static constexpr int kGraphKey = 7;
-    mutable const void* graph_key_[kGraphKey] = {};
-    // the several-column path: workspace and control block in mrhs_, one graph per batch in mgraphs_
-    using MultiRhsKey = typename Base::MultiRhsKey;
-    mutable typename Base::MultiRhsState mrhs_;
+    // the several-column path: workspace and control block in mrhs_, Hessenberg and fin here
+    mutable typename Base::FusedState mrhs_;
     mutable std::unique_ptr<Dense> mhess_;
     mutable array<std::uint64_t> mfin_;
-    mutable std::vector<b200_graph*> mgraphs_;
 };
 
 }  // namespace solver
