@@ -1,48 +1,24 @@
-/* TEST INFRASTRUCTURE ONLY.  The host-memory mock of mock_base.c plus sequential restatements of the
- * fused GMRES entry points (ginkgo_b200/csrc/fused_gmres.cu, b200_gmres_fused_multi_dot_*,
- * b200_gmres_fused_block_apply_*, b200_csr_spmv_dot2_*), so that solver::Gmres::try_fused -- capture,
- * replay of one graph per batch, polling of the control block, the host-issued restart -- runs on the
- * CPU.  Sums run sequentially from row 0, as the oracle's, so the fused path must give the loop's bits.
- * The Givens update, the multi-dot and the block-Jacobi apply call what the loop calls (the oracle's
- * hessenberg_qr, the mock's multi_dot and simple_apply).  mock_base.c is compiled as part of this file;
- * its b200_graph_launch is kept under another name and replays the operations it knows.
- * Built by tests/mock_gmres_build.py. */
-#define b200_graph_launch mock_base_graph_launch
-#include "mock_base.c"
-#undef b200_graph_launch
-
-void orc_common_gmres_hessenberg_qr_f64(int64_t, double*, int64_t, double*, int64_t, double*, double*, int64_t,
-                                        double*, int64_t, int64_t, uint64_t*, const uint8_t*);
-void orc_common_gmres_hessenberg_qr_f32(int64_t, float*, int64_t, float*, int64_t, float*, float*, int64_t,
-                                        float*, int64_t, int64_t, uint64_t*, const uint8_t*);
-
-enum { OP_G_SCALE = 200, OP_G_MGS, OP_G_SUB, OP_G_FINAL, OP_G_MDOT, OP_G_BLOCK, OP_G_SPMV_DOT2 };
+/* TEST INFRASTRUCTURE ONLY.  Sequential restatements of the fused GMRES entry points
+ * (ginkgo_b200/csrc/fused_gmres.cu, b200_gmres_fused_multi_dot_*, b200_gmres_fused_block_apply_*), so
+ * that solver::Gmres::try_fused -- capture, replay of one graph per batch, polling of the control block,
+ * the host-issued restart -- runs on the CPU.  Sums run sequentially from row 0, as the oracle's, so the
+ * fused path must give the loop's bits.  The Givens update, the multi-dot and the block-Jacobi apply call
+ * what the loop calls (the oracle's hessenberg_qr, the mock's multi_dot and simple_apply).  The SpMV +
+ * dots (b200_csr_spmv_dot2_*) are in mock_spmv_dot.c. */
+#include "mock.h"
 
 /* the criteria of fused_common.cuh, without the finalized bit; status into ctl[0] and the stop byte */
-static void mock_gmres_check(double tau_le_thr, int32_t* ctl, uint8_t* stop)
+static void mock_gmres_check(int converged, int32_t* ctl, uint8_t* stop)
 {
     const int32_t iter = ++ctl[1];
-    const int32_t max_iters = ctl[2], res_kind = ctl[3], iter_first = ctl[4];
-    uint8_t status = 0, id = 1;
-    for (int k = 0; k < 2 && status == 0; ++k) {
-        const int is_it = (k == 0) == (iter_first != 0);
-        if (is_it) {
-            if (max_iters < 0) continue;
-            if (iter >= max_iters) status = (uint8_t)(id & 0x3f);
-            ++id;
-        } else {
-            if (!res_kind) continue;
-            if (tau_le_thr != 0) status = (uint8_t)(0x80 | (id & 0x3f));
-            ++id;
-        }
-    }
+    const uint8_t status = mock_criteria_status(iter, ctl, converged, 0);
     if (status) {
         ctl[0] = status;
         stop[0] = status;
     }
 }
 
-#define MOCK_FUSED_GMRES(V, VT, VID, SQRT)                                                             \
+#define MOCK_FUSED_GMRES(V, VT, SQRT)                                                                  \
     static void mock_g_scale_##V(int64_t n, VT* v, VT* z, const VT* d, const VT* sc, const int32_t* ctl, \
                                  int divide)                                                           \
     {                                                                                                  \
@@ -66,7 +42,7 @@ static void mock_gmres_check(double tau_le_thr, int32_t* ctl, uint8_t* stop)
     }                                                                                                  \
     /* the final pass when hcol != NULL (the sub pass otherwise); p: w krylov coef haux hcol gsin gcos \
      * rnorm rnc fin stop sc ctl */                                                                    \
-    static void mock_g_sub_##V(int64_t n, int64_t first, int64_t j, void** p)                          \
+    static void mock_g_sub_##V(int64_t n, int64_t first, int64_t j, void* const* p)                    \
     {                                                                                                  \
         VT *w = (VT*)p[0], *hcol = (VT*)p[4], *sc = (VT*)p[11];                                        \
         const VT *K = (const VT*)p[1], *coef = (const VT*)p[2], *haux = (const VT*)p[3];               \
@@ -88,6 +64,26 @@ static void mock_gmres_check(double tau_le_thr, int32_t* ctl, uint8_t* stop)
         orc_common_gmres_hessenberg_qr_##V(1, (VT*)p[5], 1, (VT*)p[6], 1, rnorm, (VT*)p[8], 1, hcol, 1, j, \
                                            (uint64_t*)p[9], (const uint8_t*)p[10]);                    \
         mock_gmres_check(rnorm[0] <= sc[2], ctl, (uint8_t*)p[10]);                                     \
+    }                                                                                                  \
+    static b200_status replay_scale_##V(b200_ctx* ctx, const mock_op* op)                              \
+    {                                                                                                  \
+        (void)ctx;                                                                                     \
+        void* const* p = op->p;                                                                        \
+        mock_g_scale_##V(op->n[0], p[0], p[1], p[2], p[3], p[4], op->i[0]);                            \
+        return B200_OK;                                                                                \
+    }                                                                                                  \
+    static b200_status replay_mgs_##V(b200_ctx* ctx, const mock_op* op)                                \
+    {                                                                                                  \
+        (void)ctx;                                                                                     \
+        void* const* p = op->p;                                                                        \
+        mock_g_mgs_##V(op->n[0], p[0], p[1], p[2], p[3], op->n[1], p[4]);                              \
+        return B200_OK;                                                                                \
+    }                                                                                                  \
+    static b200_status replay_sub_##V(b200_ctx* ctx, const mock_op* op)                                \
+    {                                                                                                  \
+        (void)ctx;                                                                                     \
+        mock_g_sub_##V(op->n[0], op->n[1], op->n[2], op->p);                                           \
+        return B200_OK;                                                                                \
     }                                                                                                  \
     int64_t b200_gmres_fused_work_size_##V(const b200_ctx* ctx, int64_t krylov_dim)                    \
     {                                                                                                  \
@@ -115,7 +111,7 @@ static void mock_gmres_check(double tau_le_thr, int32_t* ctl, uint8_t* stop)
                                            const VT* sc, const int32_t* ctl, int32_t divide)           \
     {                                                                                                  \
         if (ctx->capture) {                                                                            \
-            mock_op* op = mock_new_op(ctx, OP_G_SCALE, VID);                                           \
+            mock_op* op = mock_new_op(ctx, replay_scale_##V);                                          \
             op->p[0] = v; op->p[1] = z; op->p[2] = (void*)inv_diag; op->p[3] = (void*)sc;              \
             op->p[4] = (void*)ctl; op->n[0] = n; op->i[0] = divide;                                    \
             return B200_OK;                                                                            \
@@ -130,7 +126,7 @@ static void mock_gmres_check(double tau_le_thr, int32_t* ctl, uint8_t* stop)
     {                                                                                                  \
         (void)work;                                                                                    \
         if (ctx->capture) {                                                                            \
-            mock_op* op = mock_new_op(ctx, OP_G_MGS, VID);                                             \
+            mock_op* op = mock_new_op(ctx, replay_mgs_##V);                                            \
             op->p[0] = w; op->p[1] = (void*)v_prev; op->p[2] = (void*)v_i; op->p[3] = hcol;            \
             op->p[4] = (void*)ctl; op->n[0] = n; op->n[1] = i;                                         \
             return B200_OK;                                                                            \
@@ -143,13 +139,12 @@ static void mock_gmres_check(double tau_le_thr, int32_t* ctl, uint8_t* stop)
                                            void* const* ptrs)                                          \
     {                                                                                                  \
         if (ctx->capture) {                                                                            \
-            mock_op* op = mock_new_op(ctx, OP_G_SUB, VID);                                             \
-            void** keep = (void**)malloc(13 * sizeof(void*)); /* lives as long as the graph */         \
-            memcpy(keep, ptrs, 13 * sizeof(void*));                                                    \
-            op->p[0] = keep; op->n[0] = n; op->n[1] = first; op->n[2] = j;                             \
+            mock_op* op = mock_new_op(ctx, replay_sub_##V);                                            \
+            memcpy(op->p, ptrs, 13 * sizeof(void*));                                                   \
+            op->n[0] = n; op->n[1] = first; op->n[2] = j;                                              \
             return B200_OK;                                                                            \
         }                                                                                              \
-        mock_g_sub_##V(n, first, j, (void**)ptrs);                                                     \
+        mock_g_sub_##V(n, first, j, ptrs);                                                             \
         ctx->launches++;                                                                               \
         return B200_OK;                                                                                \
     }                                                                                                  \
@@ -170,33 +165,39 @@ static void mock_gmres_check(double tau_le_thr, int32_t* ctl, uint8_t* stop)
                        stop, sc, ctl};                                                                 \
         return mock_g_sub_call_##V(ctx, n, first, j, p);                                               \
     }                                                                                                  \
+    static b200_status replay_multi_dot_##V(b200_ctx* ctx, const mock_op* op);                         \
     b200_status b200_gmres_fused_multi_dot_##V(b200_ctx* ctx, int64_t n, int64_t num_bases,            \
                                                const VT* krylov, const VT* w, VT* hcol,                \
                                                const int32_t* ctl, VT* work)                           \
     {                                                                                                  \
         (void)work;                                                                                    \
         if (ctx->capture) {                                                                            \
-            mock_op* op = mock_new_op(ctx, OP_G_MDOT, VID);                                            \
+            mock_op* op = mock_new_op(ctx, replay_multi_dot_##V);                                      \
             op->p[0] = (void*)krylov; op->p[1] = (void*)w; op->p[2] = hcol; op->p[3] = (void*)ctl;     \
             op->n[0] = n; op->n[1] = num_bases;                                                        \
             return B200_OK;                                                                            \
         }                                                                                              \
         if (ctl[0] != 0) return B200_OK;                                                               \
         return b200_gmres_multi_dot_##V(ctx, n, 1, num_bases, krylov, 1, w, 1, hcol, 1);               \
+    }                                                                                                  \
+    static b200_status replay_multi_dot_##V(b200_ctx* ctx, const mock_op* op)                          \
+    {                                                                                                  \
+        void* const* p = op->p;                                                                        \
+        return b200_gmres_fused_multi_dot_##V(ctx, op->n[0], op->n[1], p[0], p[1], p[2], p[3], NULL);  \
     }
-MOCK_FUSED_GMRES(f64, double, 0, sqrt)
-MOCK_FUSED_GMRES(f32, float, 1, sqrtf)
+MOCK_FUSED_GMRES(f64, double, sqrt)
+MOCK_FUSED_GMRES(f32, float, sqrtf)
 
 /* the ctl-aware block-Jacobi apply: the mock's simple_apply (plain or adaptive) unless stopped */
-#define MOCK_FUSED_GMRES_BLOCK(V, VT, VID, I, IT, IID)                                                 \
+#define MOCK_FUSED_GMRES_BLOCK(V, VT, I, IT)                                                           \
+    static b200_status replay_block_apply_##V##_##I(b200_ctx* ctx, const mock_op* op);                 \
     b200_status b200_gmres_fused_block_apply_##V##_##I(                                                \
         b200_ctx* ctx, int64_t num_blocks, int32_t max_block_size, int64_t block_offset,               \
         int64_t group_offset, int32_t group_power, const uint8_t* block_precisions,                    \
         const IT* block_pointers, const VT* blocks, const VT* b, VT* x, const int32_t* ctl)            \
     {                                                                                                  \
         if (ctx->capture) {                                                                            \
-            mock_op* op = mock_new_op(ctx, OP_G_BLOCK, VID);                                           \
-            op->it = IID;                                                                              \
+            mock_op* op = mock_new_op(ctx, replay_block_apply_##V##_##I);                              \
             op->p[0] = (void*)block_precisions; op->p[1] = (void*)block_pointers;                      \
             op->p[2] = (void*)blocks; op->p[3] = (void*)b; op->p[4] = x; op->p[5] = (void*)ctl;        \
             op->n[0] = num_blocks; op->n[1] = block_offset; op->n[2] = group_offset;                   \
@@ -212,101 +213,14 @@ MOCK_FUSED_GMRES(f32, float, 1, sqrtf)
         return b200_jacobi_simple_apply_##V##_##I(ctx, num_blocks, max_block_size, block_offset,       \
                                                   group_offset, group_power, block_pointers, blocks,   \
                                                   b, 1, 1, x, 1);                                      \
-    }
-MOCK_FUSED_GMRES_BLOCK(f64, double, 0, i32, int32_t, 0)
-MOCK_FUSED_GMRES_BLOCK(f64, double, 0, i64, int64_t, 1)
-MOCK_FUSED_GMRES_BLOCK(f32, float, 1, i32, int32_t, 0)
-MOCK_FUSED_GMRES_BLOCK(f32, float, 1, i64, int64_t, 1)
-
-/* c = A b, *dot_out = w . c and (dot2_out) *dot2_out = c . c over the rows; no-op once the solver stopped */
-#define MOCK_G_SPMV_DOT2(V, VT, VID, I, IT, IID)                                                       \
-    static void mock_g_spmv_dot2_##V##_##I(int64_t num_rows, const IT* rp, const IT* ci, const VT* va, \
-                                           const VT* b, VT* c, const VT* w, VT* dot_out, VT* dot2_out, \
-                                           const int32_t* ctl)                                         \
-    {                                                                                                  \
-        if (ctl && ctl[0] != 0) return;                                                                \
-        VT dot = 0, dot2 = 0;                                                                          \
-        for (int64_t r = 0; r < num_rows; ++r) {                                                       \
-            VT sum = 0;                                                                                \
-            for (int64_t k = rp[r]; k < (int64_t)rp[r + 1]; ++k) sum += va[k] * b[ci[k]];              \
-            c[r] = sum;                                                                                \
-            dot += w[r] * sum;                                                                         \
-            dot2 += sum * sum;                                                                         \
-        }                                                                                              \
-        *dot_out = dot;                                                                                \
-        if (dot2_out) *dot2_out = dot2;                                                                \
     }                                                                                                  \
-    b200_status b200_csr_spmv_dot2_##V##_##I(b200_ctx* ctx, const b200_csr_plan* plan,                 \
-                                             int64_t num_rows, int64_t num_cols, int64_t nnz,          \
-                                             const IT* row_ptrs, const IT* col_idxs, const VT* values, \
-                                             const VT* b, VT* c, const VT* w, VT* dot_out,             \
-                                             VT* dot2_out, VT* work, const int32_t* ctl)               \
+    static b200_status replay_block_apply_##V##_##I(b200_ctx* ctx, const mock_op* op)                  \
     {                                                                                                  \
-        (void)plan; (void)num_cols; (void)nnz; (void)work;                                             \
-        if (ctx->capture) {                                                                            \
-            mock_op* op = mock_new_op(ctx, OP_G_SPMV_DOT2, VID);                                       \
-            op->it = IID;                                                                              \
-            op->p[0] = (void*)row_ptrs; op->p[1] = (void*)col_idxs; op->p[2] = (void*)values;          \
-            op->p[3] = (void*)b; op->p[4] = c; op->p[5] = (void*)w; op->p[6] = dot_out;                \
-            op->p[7] = dot2_out; op->p[8] = (void*)ctl; op->n[0] = num_rows;                           \
-            return B200_OK;                                                                            \
-        }                                                                                              \
-        mock_g_spmv_dot2_##V##_##I(num_rows, row_ptrs, col_idxs, values, b, c, w, dot_out, dot2_out,   \
-                                   ctl);                                                               \
-        ctx->launches++;                                                                               \
-        return B200_OK;                                                                                \
+        void* const* p = op->p;                                                                        \
+        return b200_gmres_fused_block_apply_##V##_##I(ctx, op->n[0], op->i[0], op->n[1], op->n[2],     \
+                                                      op->i[1], p[0], p[1], p[2], p[3], p[4], p[5]);   \
     }
-MOCK_G_SPMV_DOT2(f64, double, 0, i32, int32_t, 0)
-MOCK_G_SPMV_DOT2(f64, double, 0, i64, int64_t, 1)
-MOCK_G_SPMV_DOT2(f32, float, 1, i32, int32_t, 0)
-MOCK_G_SPMV_DOT2(f32, float, 1, i64, int64_t, 1)
-
-b200_status b200_graph_launch(b200_ctx* ctx, b200_graph* graph)
-{
-    for (int k = 0; k < graph->g.count; ++k) {
-        mock_op* op = &graph->g.ops[k];
-        const int f32 = op->vt == 1;
-        void** p = op->p;
-        b200_status st = B200_OK;
-        switch (op->kind) {
-        case OP_G_SCALE:
-            if (f32) mock_g_scale_f32(op->n[0], p[0], p[1], p[2], p[3], p[4], op->i[0]);
-            else mock_g_scale_f64(op->n[0], p[0], p[1], p[2], p[3], p[4], op->i[0]);
-            break;
-        case OP_G_MGS:
-            if (f32) mock_g_mgs_f32(op->n[0], p[0], p[1], p[2], p[3], op->n[1], p[4]);
-            else mock_g_mgs_f64(op->n[0], p[0], p[1], p[2], p[3], op->n[1], p[4]);
-            break;
-        case OP_G_SUB:
-            if (f32) mock_g_sub_f32(op->n[0], op->n[1], op->n[2], (void**)p[0]);
-            else mock_g_sub_f64(op->n[0], op->n[1], op->n[2], (void**)p[0]);
-            break;
-        case OP_G_MDOT:
-            st = f32 ? b200_gmres_fused_multi_dot_f32(ctx, op->n[0], op->n[1], p[0], p[1], p[2], p[3], NULL)
-                     : b200_gmres_fused_multi_dot_f64(ctx, op->n[0], op->n[1], p[0], p[1], p[2], p[3], NULL);
-            break;
-        case OP_G_BLOCK:
-#define G_BLOCK(V, I) b200_gmres_fused_block_apply_##V##_##I(ctx, op->n[0], op->i[0], op->n[1], op->n[2], op->i[1], p[0], p[1], p[2], p[3], p[4], p[5])
-            st = f32 ? (op->it ? G_BLOCK(f32, i64) : G_BLOCK(f32, i32)) : (op->it ? G_BLOCK(f64, i64) : G_BLOCK(f64, i32));
-#undef G_BLOCK
-            break;
-        case OP_G_SPMV_DOT2:
-#define G_SD2(V, I) mock_g_spmv_dot2_##V##_##I(op->n[0], p[0], p[1], p[2], p[3], p[4], p[5], p[6], p[7], p[8])
-            if (f32) { if (op->it) G_SD2(f32, i64); else G_SD2(f32, i32); }
-            else { if (op->it) G_SD2(f64, i64); else G_SD2(f64, i32); }
-#undef G_SD2
-            break;
-        default: {  /* an operation of mock_base.c */
-            b200_graph one;
-            one.g.ops = op;
-            one.g.count = one.g.cap = 1;
-            st = mock_base_graph_launch(ctx, &one);
-            if (st != B200_OK) return st;
-            continue;
-        }
-        }
-        if (st != B200_OK) return st;
-        ctx->launches++;
-    }
-    return B200_OK;
-}
+MOCK_FUSED_GMRES_BLOCK(f64, double, i32, int32_t)
+MOCK_FUSED_GMRES_BLOCK(f64, double, i64, int64_t)
+MOCK_FUSED_GMRES_BLOCK(f32, float, i32, int32_t)
+MOCK_FUSED_GMRES_BLOCK(f32, float, i64, int64_t)

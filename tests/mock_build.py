@@ -1,15 +1,18 @@
 """TEST INFRASTRUCTURE ONLY: builds the C++ host layer (ginkgo_b200/host/capi.cpp) together with
 tests/mock -- the host-memory stand-in for the C ABI whose kernel entry points forward to the
-oracle -- into one DSO and wraps it for ginkgo_b200.api.  Used by tests/test_host_cpu.py and, with
+oracle, with the fused solver kernels restated by hand -- into one DSO and wraps it for
+ginkgo_b200.api.  Used by tests/test_host_cpu.py, the tests/test_fused_*_cpu.py files and, with
 B200_TEST_SELFCHECK=1, as a stand-in for the GPU executor when the bodies of the gpu tests are
 checked on a machine without a GPU."""
 import ctypes
+import glob
 import os
 import subprocess
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+MOCK_DIR = os.path.join(ROOT, "tests", "mock")
 
 
 class CpuExec:
@@ -30,19 +33,29 @@ class CpuExec:
 
 
 def build_mock_objects(d, sanitize=()):
-    """mock_base.c + the generated forwarders, compiled into `d`; returns the object files"""
+    """the handwritten tests/mock/*.c + the generated forwarders, compiled into `d`; returns the object
+    files"""
     inc = os.path.join(ROOT, "include")
-    gen = os.path.join(d, "mock_gen.c")
-    subprocess.run(["python", os.path.join(ROOT, "tests", "mock", "gen_mock.py"),
-                    os.path.join(inc, "ginkgo_b200.h"), os.path.join(ROOT, "oracle", "liboracle.so"),
-                    os.path.join(ROOT, "tests", "mock", "mock_base.c"), gen], check=True,
-                   capture_output=True)
-    objs = []
-    for src in (os.path.join(ROOT, "tests", "mock", "mock_base.c"), gen):
+
+    def compile_c(src):
         o = os.path.join(d, os.path.basename(src) + ".o")
         subprocess.run(["gcc", "-O1", "-fPIC", "-I" + inc, "-c", src, "-o", o] + list(sanitize), check=True)
-        objs.append(o)
-    return objs
+        return o
+
+    objs = [compile_c(src) for src in sorted(glob.glob(os.path.join(MOCK_DIR, "*.c")))]
+    # gen_mock.py forwards or stubs every entry point these objects do not define
+    handwritten = set()
+    for o in objs:
+        for line in subprocess.run(["nm", "-g", "--defined-only", o], check=True, capture_output=True,
+                                   text=True).stdout.splitlines():
+            parts = line.split()
+            if len(parts) == 3 and parts[2].startswith("b200_"):
+                handwritten.add(parts[2])
+    gen = os.path.join(d, "mock_gen.c")
+    subprocess.run(["python", os.path.join(MOCK_DIR, "gen_mock.py"), os.path.join(inc, "ginkgo_b200.h"),
+                    os.path.join(ROOT, "oracle", "liboracle.so"), gen] + sorted(handwritten), check=True,
+                   capture_output=True)
+    return objs + [compile_c(gen)]
 
 
 def link_args():
@@ -61,7 +74,9 @@ def build_mock_executable(d, source, name):
 def build_mock_host(d):
     from ginkgo_b200 import api
     # B200_MOCK_SANITIZE=1: build the host layer + mock with ASan / UBSan; run pytest with
-    # LD_PRELOAD="$(g++ -print-file-name=libasan.so) $(g++ -print-file-name=libstdc++.so)"
+    # LD_PRELOAD="$(g++ -print-file-name=libasan.so) $(g++ -print-file-name=libstdc++.so)" and
+    # ASAN_OPTIONS=detect_leaks=0 (the preload also reaches gcc and python, whose exit-time leaks
+    # would fail the build)
     san = (["-fsanitize=address,undefined", "-fno-omit-frame-pointer", "-g"]
            if os.environ.get("B200_MOCK_SANITIZE") == "1" else [])
     objs = build_mock_objects(d, san)

@@ -16,8 +16,7 @@ FIN_CONV_2 = 0x80 | 0x40 | 2  # converged by the residual criterion, second of I
 @pytest.fixture(scope="module")
 def host(tmp_path_factory):
     from ginkgo_b200 import api
-    from tests.mock_bicgstab_mrhs_build import build_mock_host
-    from tests.mock_build import CpuExec
+    from tests.mock_build import CpuExec, build_mock_host
     lib = build_mock_host(str(tmp_path_factory.mktemp("mock_bicgstab_mrhs")))
     saved = api._HOST_LIB
     api._HOST_LIB = lib

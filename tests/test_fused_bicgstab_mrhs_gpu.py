@@ -7,17 +7,15 @@ with -fmad=false, numpy in the value type rounds as the device does); sums on sm
 be exact; sums on random data must lie within gamma_h * sum |t| of math.fsum, which bounds any
 summation order.  Every vector is n x k row-major (stride k).
 
-B200_TEST_SELFCHECK=1 runs the same bodies on the host-memory mock of
-tests/mock/mock_fused_bicgstab_mrhs.c."""
-import os
-
+B200_TEST_SELFCHECK=1 runs the same bodies on the host-memory mock of tests/mock."""
 import numpy as np
 import pytest
 
 from tests import helpers as H
 from tests.helpers import IT, VT
 from tests.test_fused_bicgstab_gpu import convective_arrow, true_rel_res, upwind
-from tests.test_fused_cg_gpu import Backend, arrow_inv_diag, assert_sum_within, expected_status, int_sum, tau_of
+from tests.test_fused_cg_gpu import (arrow_inv_diag, assert_sum_within, backend, dev,  # noqa: F401
+                                     expected_status, hexec, int_sum, tau_of)
 from tests.test_fused_cg_mrhs_gpu import big_case, lanes, nans, oracle_spmv
 from tests.test_parity_gpu import CSR_KINDS, csr_case
 
@@ -30,40 +28,6 @@ STOPPED = 0x40 | 1
 MID_STOPPED = 0x80 | 2     # converged at the mid check, not yet finalized
 FIN_CONV_2 = 0x80 | 0x40 | 2
 SPMV_THREADS, SPMV_CTAS_PER_SM = 256, 8  # fused_mrhs.cuh: the SpMV's block size and grid cap per SM
-
-
-@pytest.fixture(scope="module")
-def backend(tmp_path_factory):
-    from ginkgo_b200 import _cdecl, _lib
-    if os.environ.get("B200_TEST_SELFCHECK") == "1":
-        # harness self-check (no GPU): the host-memory mock stands in for the device
-        from tests.mock_bicgstab_mrhs_build import build_mock_host
-        lib = build_mock_host(str(tmp_path_factory.mktemp("fused_bicgstab_mrhs_mock")))
-        _cdecl.bind(lib, _lib.declarations())
-        be = Backend(lib, mock=True)
-    else:
-        be = Backend(_lib.lib(), mock=False)
-    yield be
-    be.close()
-
-
-@pytest.fixture
-def dev(backend):
-    yield backend
-    backend.release()
-
-
-@pytest.fixture(scope="module")
-def hexec(backend):
-    from ginkgo_b200 import api
-    if backend.mock:
-        from tests.mock_build import CpuExec
-        saved = api._HOST_LIB
-        api._HOST_LIB = backend.l
-        yield CpuExec(backend.l)
-        api._HOST_LIB = saved
-    else:
-        yield api.HostExecutor(0)
 
 
 def work(dev, vt, k):

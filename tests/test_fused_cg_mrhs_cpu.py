@@ -13,8 +13,7 @@ from tests.helpers import VT
 @pytest.fixture(scope="module")
 def host(tmp_path_factory):
     from ginkgo_b200 import api
-    from tests.mock_cg_mrhs_build import build_mock_host
-    from tests.mock_build import CpuExec
+    from tests.mock_build import CpuExec, build_mock_host
     lib = build_mock_host(str(tmp_path_factory.mktemp("mock_cg_mrhs")))
     saved = api._HOST_LIB
     api._HOST_LIB = lib

@@ -1,5 +1,5 @@
-"""solver::Gmres::try_fused on the host-memory mock (tests/mock/mock_fused_gmres.c): one graph per batch
-of check_every iterations, polling of the control block, the host-issued restart and the final update
+"""solver::Gmres::try_fused on the host-memory mock (tests/mock): one graph per batch of
+check_every iterations, polling of the control block, the host-issued restart and the final update
 run on the CPU.  The mock's restatements and the kernel-by-kernel loop both sum their dots and norms
 sequentially from row 0, so the fused path must give the loop's iterations, status and bits of x."""
 import numpy as np
@@ -13,8 +13,7 @@ from tests.test_fused_bicgstab_cpu import convection_diffusion
 @pytest.fixture(scope="module")
 def host(tmp_path_factory):
     from ginkgo_b200 import api
-    from tests.mock_build import CpuExec
-    from tests.mock_gmres_build import build_mock_host
+    from tests.mock_build import CpuExec, build_mock_host
     lib = build_mock_host(str(tmp_path_factory.mktemp("mock_gmres")))
     saved = api._HOST_LIB
     api._HOST_LIB = lib

@@ -5,36 +5,18 @@ solver against the device loop and the oracle.
 Assertions as in tests/test_fused_bicgstab_gpu.py: element-wise updates and the scalars derived from
 given sums BIT FOR BIT, reductions on small-integer data for EQUALITY with the exact sum, reductions on
 random data against math.fsum within gamma_h * sum |t|."""
-import os
-
 import numpy as np
 import pytest
 
 from tests import helpers as H
 from tests.helpers import VT
 from tests.test_fused_bicgstab_gpu import SYSTEMS, convective_arrow, true_rel_res, upwind
-from tests.test_fused_cg_gpu import (STOPPED, VTS, Backend, arrow_inv_diag, assert_sum_within, dev,  # noqa: F401
-                                     hexec, nans)
+from tests.test_fused_cg_gpu import (STOPPED, VTS, arrow_inv_diag, assert_sum_within, backend,  # noqa: F401
+                                     dev, hexec, nans)
 
 pytestmark = pytest.mark.gpu
 
 SC, CTL = 8, 8  # sc: 0 ||w|| of the last final pass, 1 tau0, 2 threshold
-
-
-@pytest.fixture(scope="module")
-def backend(tmp_path_factory):
-    """as in test_fused_cg_gpu.py; B200_TEST_SELFCHECK=1 runs the bodies on the host-memory mock that
-    restates the fused GMRES entry points (tests/mock/mock_fused_gmres.c)"""
-    from ginkgo_b200 import _cdecl, _lib
-    if os.environ.get("B200_TEST_SELFCHECK") == "1":
-        from tests.mock_gmres_build import build_mock_host
-        lib = build_mock_host(str(tmp_path_factory.mktemp("fused_gmres_mock")))
-        _cdecl.bind(lib, _lib.declarations())
-        be = Backend(lib, mock=True)
-    else:
-        be = Backend(_lib.lib(), mock=False)
-    yield be
-    be.close()
 
 
 def vec(vt, n, data, seed):

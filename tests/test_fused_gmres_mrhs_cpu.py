@@ -1,5 +1,5 @@
-"""solver::Gmres::try_fused_multi_rhs on the host-memory mock (tests/mock/mock_fused_gmres_mrhs.c): one graph
-per batch of check_every iterations, polling of the control block, the per-column statuses and the restart
+"""solver::Gmres::try_fused_multi_rhs on the host-memory mock (tests/mock): one graph per
+batch of check_every iterations, polling of the control block, the per-column statuses and the restart
 issued on all k columns run on the CPU.  The mock's restatements and the kernel-by-kernel loop both sum
 every column's dots and norms over the rows in order, so the fused path must give the loop's iterations,
 per-column statuses and bits of x."""
@@ -17,8 +17,7 @@ ITER_1 = 0x40 | 1          # the Iteration limit, finalized
 @pytest.fixture(scope="module")
 def host(tmp_path_factory):
     from ginkgo_b200 import api
-    from tests.mock_build import CpuExec
-    from tests.mock_gmres_mrhs_build import build_mock_host
+    from tests.mock_build import CpuExec, build_mock_host
     lib = build_mock_host(str(tmp_path_factory.mktemp("mock_gmres_mrhs")))
     saved = api._HOST_LIB
     api._HOST_LIB = lib

@@ -7,16 +7,15 @@ compared BIT FOR BIT (the library is built with -fmad=false, numpy in the value 
 does); sums on small-integer data must be exact; sums on random data must lie within gamma_h * sum |t| of
 math.fsum.  Every vector is n x k row-major (stride k); column c of basis i is K[i n + r, c].
 
-B200_TEST_SELFCHECK=1 runs the same bodies on the host-memory mock of tests/mock/mock_fused_gmres_mrhs.c."""
-import os
-
+B200_TEST_SELFCHECK=1 runs the same bodies on the host-memory mock of tests/mock."""
 import numpy as np
 import pytest
 
 from tests import helpers as H
 from tests.helpers import VT
 from tests.test_fused_bicgstab_gpu import SYSTEMS, true_rel_res, upwind
-from tests.test_fused_cg_gpu import Backend, arrow_inv_diag, assert_sum_within, int_sum
+from tests.test_fused_cg_gpu import (arrow_inv_diag, assert_sum_within, backend, dev, hexec,  # noqa: F401
+                                     int_sum)
 from tests.test_fused_cg_mrhs_gpu import nans, oracle_spmv
 from tests.test_fused_gmres_gpu import assert_norm_within, givens_ref
 
@@ -28,40 +27,6 @@ CTL = 8
 STOPPED = 0x40 | 1        # a stopped column (Iteration, finalized)
 CONV_2 = 0x80 | 0x40 | 2  # converged by the residual criterion (second of Iteration first), finalized
 THREADS, STEP_CTAS_PER_SM = 512, 4  # fused_common.cuh / fused_mrhs.cuh: the passes' block size and grid cap
-
-
-@pytest.fixture(scope="module")
-def backend(tmp_path_factory):
-    from ginkgo_b200 import _cdecl, _lib
-    if os.environ.get("B200_TEST_SELFCHECK") == "1":
-        # harness self-check (no GPU): the host-memory mock stands in for the device
-        from tests.mock_gmres_mrhs_build import build_mock_host
-        lib = build_mock_host(str(tmp_path_factory.mktemp("fused_gmres_mrhs_mock")))
-        _cdecl.bind(lib, _lib.declarations())
-        be = Backend(lib, mock=True)
-    else:
-        be = Backend(_lib.lib(), mock=False)
-    yield be
-    be.close()
-
-
-@pytest.fixture
-def dev(backend):
-    yield backend
-    backend.release()
-
-
-@pytest.fixture(scope="module")
-def hexec(backend):
-    from ginkgo_b200 import api
-    if backend.mock:
-        from tests.mock_build import CpuExec
-        saved = api._HOST_LIB
-        api._HOST_LIB = backend.l
-        yield CpuExec(backend.l)
-        api._HOST_LIB = saved
-    else:
-        yield api.HostExecutor(0)
 
 
 def work(dev, vt, k, kd=31):

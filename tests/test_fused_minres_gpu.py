@@ -9,36 +9,17 @@ reductions on random data against math.fsum within gamma_h * sum |t|.
 
 B200_TEST_SELFCHECK=1 runs the same bodies on the host-memory mock of tests/mock; the asserts about
 the device's launch shapes are skipped there, each marked "mock:"."""
-import os
-
 import numpy as np
 import pytest
 
 from tests import helpers as H
 from tests.helpers import IT, VT
-from tests.test_fused_cg_gpu import (ITS, STOPPED, VARIANTS, VTS, Backend, Mat, arrow, arrow_inv_diag,  # noqa: F401
-                                     assert_sum_within, dev, exact_limit, exact_spmv, expected_status, hexec,
-                                     int_sum, nans, spmv_case, step_sizes)
+from tests.test_fused_cg_gpu import (ITS, STOPPED, VARIANTS, VTS, Mat, arrow, arrow_inv_diag,  # noqa: F401
+                                     assert_sum_within, backend, dev, exact_limit, exact_spmv, expected_status,
+                                     hexec, int_sum, nans, spmv_case, step_sizes)
 from tests.test_parity_gpu import CSR_KINDS
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def backend(tmp_path_factory):
-    """as in test_fused_cg_gpu.py (its `dev` and `hexec` fixtures build on this one); the self-check
-    uses the mock that restates the fused MINRES entry points"""
-    from ginkgo_b200 import _cdecl, _lib
-    if os.environ.get("B200_TEST_SELFCHECK") == "1":
-        from tests.mock_minres_build import build_mock_host
-        lib = build_mock_host(str(tmp_path_factory.mktemp("fused_minres_mock")))
-        _cdecl.bind(lib, _lib.declarations())
-        be = Backend(lib, mock=True)
-    else:
-        be = Backend(_lib.lib(), mock=False)
-    yield be
-    be.close()
-
 
 SC, CTL = 16, 8
 # sc: 0 alpha 1 beta 2 gamma 3 delta 4 tau0 5 threshold 6 tau 7 eta 8 eta_next 9 cos_prev 10 cos
