@@ -88,6 +88,15 @@ constexpr int kWarp = 32;
 
 __host__ __device__ inline int64_t ceildiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// Slots of b200_ctx::counters that the fused solvers' grid-wide sums take their tickets from.  The same
+// 256 counters serve the BLAS-1 reductions (dense_blas1.cu: slot t for column tile t of a batch, so any
+// of 0..255) and the unfused GMRES multi-dot (slot 0).  Sharing is safe because every kernel that takes
+// a ticket resets its slot to 0 in the CTA that takes the last one, and every user launches on
+// ctx->stream (directly or in a graph captured on it), so no two kernels hold a slot at the same time.
+constexpr int kSpmvDotCounter = 1;   // the SpMV's dot epilogue (csr::DotArgs, mrhs::spmv_mdot)
+constexpr int kStepCounter = 2;      // the fused step kernels
+constexpr int kMultiDotCounter = 3;  // the multi-dot that honours ctl (GMRES's fused CGS / CGS2)
+
 // stopping_status bit layout (include/ginkgo/core/stop/stopping_status.hpp)
 constexpr uint8_t kConvergedMask = 1u << 7;
 constexpr uint8_t kFinalizedMask = 1u << 6;

@@ -299,5 +299,39 @@ b200_status launch_planned(b200_ctx* ctx, const b200_csr_plan* plan, Variant v, 
     return B200_OK;
 }
 
+// the SpMV + dot on a matrix without rows: there are no tiles, so no SpMV kernel runs and writes the sums
+template <typename V>
+__global__ void empty_dot_kernel(V* dot_out, V* dot2_out, const int32_t* ctl)
+{
+    if (ctl && ctl[0] != 0) return;
+    *dot_out = V(0);
+    if (dot2_out) *dot2_out = V(0);
+}
+
+// The SpMV + dot entry points of the fused solvers (b200_csr_spmv_{dot,dot2,sub_dot}_*): c = A b, or
+// c = alpha A b + beta c (ADVANCED), and the sums of DOT into dot_out (and dot2_out unless it is null, w
+// the second operand of kDotW2) through the plan's variant, which must not be kSlab.  `work` holds the
+// per-CTA partials; ctl may be null.  A matrix without rows gets zero sums.
+template <typename V, typename I, bool ADVANCED, int DOT>
+b200_status launch_spmv_dot(b200_ctx* ctx, const b200_csr_plan* plan, int64_t num_rows, int64_t nnz,
+                            const I* row_ptrs, const I* col_idxs, const V* values, const V* alpha, const V* b,
+                            const V* beta, V* c, const V* w, V* dot_out, V* dot2_out, V* work, const int32_t* ctl)
+{
+    B200_REQUIRE(ctx && plan && (DOT != kDotW2 || w) && dot_out && work, "null argument (a plan is required)");
+    B200_REQUIRE(plan->num_rows == num_rows && plan->nnz == nnz, "plan does not match");
+    const Variant v = pick_variant(col_idxs, values, plan);
+    B200_REQUIRE(v != kSlab, "col_idxs/values must be 32-byte aligned");
+    if (num_rows == 0) {
+        empty_dot_kernel<V><<<1, 1, 0, ctx->stream>>>(dot_out, dot2_out, ctl);
+        B200_LAUNCH_CHECK(ctx);
+        return B200_OK;
+    }
+    DotArgs<V> dot{work, ctx->counters + kSpmvDotCounter, dot_out, ctl};
+    dot.w = w;
+    dot.result2 = dot2_out;
+    return launch_planned<V, I, ADVANCED, DOT>(ctx, plan, v, nnz, row_ptrs, col_idxs, values, alpha, b, 1, beta, c,
+                                               1, dot);
+}
+
 }  // namespace csr
 }  // namespace b200

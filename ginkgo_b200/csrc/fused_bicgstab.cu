@@ -29,16 +29,15 @@
 //
 // Scalars  sc[16]: 0 rho, 1 prev_rho, 2 beta (rr.v, then t.t), 3 ||r||^2, 4 tau0 (baseline norm),
 //                  5 threshold = reduction_factor * tau0, 6 alpha, 7 omega, 8 gamma, 9 ||s||^2
-// Control  ctl[8] (int32): 0 stopping_status byte (0 = running), 1 iterations done, 2 max_iters (-1 none),
-//                  3 res_kind (0 none, 1 ResidualNorm, 2 ImplicitResidualNorm), 4 iter_first,
-//                  5 finalize pending (x += alpha y still owed after a stop at the mid check)
+// Control  ctl[0..4] of fused_common.cuh; 5 finalize pending (x += alpha y still owed after a stop at the
+//                  mid check), 6..7 unused
 #include "csr_launch.cuh"
 #include "fused_common.cuh"
 
 namespace b200 {
 namespace fbicgstab {
 
-using namespace fused;  // kThreads, grid_sums, finish_scalars, ew_grid
+using namespace fused;  // kThreads, grid_sums, residual_status, finish_scalars, set_threshold, ew_grid
 
 template <typename V>
 __global__ void __launch_bounds__(kThreads)
@@ -64,23 +63,7 @@ __global__ void __launch_bounds__(kThreads)
 template <typename V>
 __device__ void mid_check(V ss, const V* sc, int32_t* ctl)
 {
-    const int32_t iter = ctl[1], max_iters = ctl[2], res_kind = ctl[3], iter_first = ctl[4];
-    const bool has_it = max_iters >= 0, has_res = res_kind != 0;
-    uint8_t status = 0;
-    uint8_t id = 1;
-    for (int k = 0; k < 2 && status == 0; ++k) {
-        const bool is_it = (k == 0) == (iter_first != 0);
-        if (is_it) {
-            if (!has_it) continue;
-            if (iter >= max_iters) status = (id & kIdMask) | kFinalizedMask;
-            ++id;
-        } else {
-            if (!has_res) continue;
-            const V tau = res_kind == 1 ? sqrt(ss) : sqrt(fabs(sc[0]));
-            if (tau <= sc[5]) status = kConvergedMask | (id & kIdMask) | kFinalizedMask;
-            ++id;
-        }
-    }
+    const uint8_t status = residual_status(ctl[1], ctl, ss, sc[0], sc[5], kFinalizedMask);
     if (status != 0) {
         ctl[0] = status;
         ctl[5] = 1;  // bicgstab::finalize is owed: step_xr pays it
@@ -163,10 +146,7 @@ __global__ void __launch_bounds__(kThreads)
             return;
         }
         if (INIT) {
-            // baseline: 0 rhs_norm (sc[4] preset to ||b||), 1 initial_resnorm, 2 absolute
-            if (baseline == 1) sc[4] = sqrt(a[1]);
-            if (baseline == 2) sc[4] = V(1);
-            sc[5] = factor * sc[4];
+            set_threshold(baseline, sqrt(a[1]), sc + 4, sc + 5, factor);
         } else {
             sc[7] = sc[2] != V(0) ? sc[8] / sc[2] : V(0);
         }
@@ -188,21 +168,8 @@ __global__ void init_scalars_kernel(V* sc, int32_t* ctl, int32_t max_iters, int3
     sc[7] = V(1);
     sc[8] = V(1);
     sc[9] = V(0);
-    ctl[0] = 0;
-    ctl[1] = -1;  // the INIT finish increments to 0
-    ctl[2] = max_iters;
-    ctl[3] = res_kind;
-    ctl[4] = iter_first;
+    start_control(ctl, max_iters, res_kind, iter_first, -1);  // the INIT finish counts to 0
     ctl[5] = 0;
-}
-
-// spmv_dot2 on a matrix without rows: there are no tiles, so no SpMV kernel runs and writes the sums
-template <typename V>
-__global__ void empty_dot2_kernel(V* dot_out, V* dot2_out, const int32_t* ctl)
-{
-    if (ctl && ctl[0] != 0) return;
-    *dot_out = V(0);
-    if (dot2_out) *dot2_out = V(0);
 }
 
 }  // namespace fbicgstab
@@ -218,15 +185,15 @@ extern "C" {
     {                                                                                             \
         B200_REQUIRE(ctx && sc && ctl && work, "null argument");                                  \
         b200::fbicgstab::init_scalars_kernel<VT><<<1, 1, 0, ctx->stream>>>(                       \
-            sc, ctl, (int32_t)(max_iters > 0x7fffffff ? 0x7fffffff : max_iters), res_kind,        \
-            iter_first);                                                                          \
+            sc, ctl, b200::fused::clamp_iters(max_iters), res_kind, iter_first);                  \
         B200_LAUNCH_CHECK(ctx);                                                                   \
         VT* zeroed[6] = {p, v, y, s, t, z};                                                       \
         for (VT * a : zeroed) B200_CUDA_CHECK(cudaMemsetAsync(a, 0, sizeof(VT) * n, ctx->stream)); \
         const int grid = b200::fused::ew_grid(ctx, n);                                            \
         b200::fbicgstab::step_xr_kernel<VT, true><<<grid, b200::fused::kThreads, 0, ctx->stream>>>( \
             n, nullptr, const_cast<VT*>(r), nullptr, nullptr, nullptr, nullptr, rr, sc, ctl,      \
-            work + (int64_t)ctx->num_sms * 4, ctx->counters + 2, baseline, reduction_factor);     \
+            b200::fused::step_partials(ctx, work), ctx->counters + b200::kStepCounter, baseline,  \
+            reduction_factor);                                                                    \
         B200_LAUNCH_CHECK(ctx);                                                                   \
         return B200_OK;                                                                           \
     }                                                                                             \
@@ -246,8 +213,8 @@ extern "C" {
     {                                                                                             \
         const int grid = b200::fused::ew_grid(ctx, n);                                            \
         b200::fbicgstab::step_s_kernel<VT><<<grid, b200::fused::kThreads, 0, ctx->stream>>>(      \
-            n, r, v, s, z, inv_diag, sc, ctl, work + (int64_t)ctx->num_sms * 4,                   \
-            ctx->counters + 2);                                                                   \
+            n, r, v, s, z, inv_diag, sc, ctl, b200::fused::step_partials(ctx, work),              \
+            ctx->counters + b200::kStepCounter);                                                  \
         B200_LAUNCH_CHECK(ctx);                                                                   \
         return B200_OK;                                                                           \
     }                                                                                             \
@@ -259,8 +226,8 @@ extern "C" {
         const int grid = b200::fused::ew_grid(ctx, n);                                            \
         b200::fbicgstab::step_xr_kernel<VT, false><<<grid, b200::fused::kThreads, 0,              \
                                                      ctx->stream>>>(                              \
-            n, x, r, s, t, y, z, const_cast<VT*>(rr), sc, ctl, work + (int64_t)ctx->num_sms * 4,  \
-            ctx->counters + 2, 0, VT(0));                                                         \
+            n, x, r, s, t, y, z, const_cast<VT*>(rr), sc, ctl,                                    \
+            b200::fused::step_partials(ctx, work), ctx->counters + b200::kStepCounter, 0, VT(0)); \
         B200_LAUNCH_CHECK(ctx);                                                                   \
         return B200_OK;                                                                           \
     }
@@ -276,21 +243,9 @@ B200_DEF_FBICGSTAB(f32, float)
         int64_t nnz, const IT* row_ptrs, const IT* col_idxs, const VT* values, const VT* b,       \
         VT* c, const VT* w, VT* dot_out, VT* dot2_out, VT* work, const int32_t* ctl)              \
     {                                                                                             \
-        B200_REQUIRE(ctx && plan && w && dot_out && work, "null argument (a plan is required)");  \
-        B200_REQUIRE(plan->num_rows == num_rows && plan->nnz == nnz, "plan does not match");      \
-        const b200::csr::Variant v = b200::csr::pick_variant(col_idxs, values, plan);             \
-        B200_REQUIRE(v != b200::csr::kSlab, "col_idxs/values must be 32-byte aligned");           \
-        if (num_rows == 0) {                                                                      \
-            b200::fbicgstab::empty_dot2_kernel<VT><<<1, 1, 0, ctx->stream>>>(dot_out, dot2_out,   \
-                                                                             ctl);                \
-            B200_LAUNCH_CHECK(ctx);                                                               \
-            return B200_OK;                                                                       \
-        }                                                                                         \
-        b200::csr::DotArgs<VT> dot{work, ctx->counters + 1, dot_out, ctl};                        \
-        dot.w = w;                                                                                \
-        dot.result2 = dot2_out;                                                                   \
-        return b200::csr::launch_planned<VT, IT, false, b200::csr::kDotW2>(                       \
-            ctx, plan, v, nnz, row_ptrs, col_idxs, values, nullptr, b, 1, nullptr, c, 1, dot);    \
+        return b200::csr::launch_spmv_dot<VT, IT, false, b200::csr::kDotW2>(                      \
+            ctx, plan, num_rows, nnz, row_ptrs, col_idxs, values, nullptr, b, nullptr, c, w,      \
+            dot_out, dot2_out, work, ctl);                                                        \
     }
 
 B200_DEF_SPMV_DOT2(f64, double, i32, int32_t)

@@ -38,9 +38,8 @@
 //                   3 ||r||^2, 4 tau0 (baseline norm), 5 threshold = reduction_factor * tau0,
 //                   6 alpha, 7 omega, 8 gamma, 9 ||s||^2
 // Status   status[k]: the reference's stopping_status byte of every column (0 = running)
-// Control  ctl[8] (int32): 0 nonzero once EVERY column has stopped, 1 iterations done, 2 max_iters
-//                   (-1 none), 3 res_kind (0 none, 1 ResidualNorm, 2 ImplicitResidualNorm),
-//                   4 iter_first, 5 some column owes its finalize (stopped at the mid check)
+// Control  ctl[0..4] of fused_common.cuh; 5 some column owes its finalize (stopped at the mid check),
+//                   6..7 unused
 #include "fused_mrhs.cuh"
 
 namespace b200 {
@@ -103,7 +102,9 @@ __global__ void __launch_bounds__(kThreads)
     if (!grid_column_sums<V, 1, kThreads>(a, k, partials, counter, tot, &is_last)) return;
     if (threadIdx.x != 0) return;
     // the mid-iteration check of every running column (core/solver/bicgstab.cpp:170-186): the top
-    // check's iteration number and rho, ||s|| as the residual norm, the finalized bit not set
+    // check's iteration number and rho, ||s|| as the residual norm, the finalized bit not set.  This and
+    // step_xr's top check restate fused::residual_status / top_check and mrhs::all_stopped: through the
+    // helpers these kernels need more registers and run slower (DESIGN.md section 4).
     const int32_t iter = ctl[1];
     bool all_stopped = true, owed = false;
     for (int c = 0; c < (int)k; ++c) {
@@ -239,19 +240,12 @@ __global__ void init_scalars_kernel(int64_t k, V* sc, uint8_t* status, int32_t* 
         status[j] = 0;
     }
     if (j == 0) {
-        ctl[0] = 0;
-        ctl[1] = -1;  // the INIT check increments to 0
-        ctl[2] = max_iters;
-        ctl[3] = res_kind;
-        ctl[4] = iter_first;
+        fused::start_control(ctl, max_iters, res_kind, iter_first, -1);  // the INIT check counts to 0
         ctl[5] = 0;
     }
 }
 
 // ---- host side of the entry points ----------------------------------------------------------------
-// `work`: the SpMV's partials (2k per CTA), then the step kernels' (2k per CTA)
-inline int64_t step_partials_offset(const b200_ctx* ctx, int64_t k) { return spmv_cap(ctx) * 2 * k; }
-
 #define B200_FBM_REQUIRE(ctx, n, k)                                                    \
     B200_REQUIRE(ctx, "null argument");                                                \
     B200_REQUIRE((n) >= 0 && (k) >= 2 && (k) <= kMaxCols, "k must be in [2, 32]")
@@ -264,10 +258,10 @@ b200_status step_xr(b200_ctx* ctx, int64_t n, int64_t k, V* x, V* r, const V* s,
     B200_REQUIRE(sc && status && ctl && work, "null argument");
     const int P = lanes_for(k);
     const int grid = rows_grid<kThreads>(n, P, step_cap(ctx));
-    V* partials = work + step_partials_offset(ctx, k);
+    V* partials = work + step_partials_offset<DotW2>(ctx, k);
 #define B200_XR(PP)                                                                                      \
     step_xr_kernel<V, PP, INIT><<<grid, kThreads, 0, ctx->stream>>>(n, k, x, r, s, t, y, z, rr, sc, status, \
-                                                                    ctl, partials, ctx->counters + 2,    \
+                                                                    ctl, partials, ctx->counters + kStepCounter, \
                                                                     baseline, factor)
     B200_MRHS_BY_LANES(P, B200_XR)
 #undef B200_XR
@@ -283,7 +277,7 @@ b200_status init(b200_ctx* ctx, int64_t n, int64_t k, const V* r, V* rr, V* p, V
     B200_FBM_REQUIRE(ctx, n, k);
     B200_REQUIRE(sc && status && ctl && work, "null argument");
     init_scalars_kernel<V><<<1, kMaxCols, 0, ctx->stream>>>(
-        k, sc, status, ctl, (int32_t)(max_iters > 0x7fffffff ? 0x7fffffff : max_iters), res_kind, iter_first);
+        k, sc, status, ctl, fused::clamp_iters(max_iters), res_kind, iter_first);
     B200_LAUNCH_CHECK(ctx);
     if (n > 0) {
         V* zeroed[6] = {p, v, y, s, t, z};
@@ -317,10 +311,10 @@ b200_status step_s(b200_ctx* ctx, int64_t n, int64_t k, const V* r, const V* v, 
     B200_REQUIRE(sc && status && ctl && work, "null argument");
     const int P = lanes_for(k);
     const int grid = rows_grid<kThreads>(n, P, step_cap(ctx));
-    V* partials = work + step_partials_offset(ctx, k);
+    V* partials = work + step_partials_offset<DotW2>(ctx, k);
 #define B200_S(PP)                                                                                      \
     step_s_kernel<V, PP><<<grid, kThreads, 0, ctx->stream>>>(n, k, r, v, s, z, inv_diag, sc, status, ctl, \
-                                                             partials, ctx->counters + 2)
+                                                             partials, ctx->counters + kStepCounter)
     B200_MRHS_BY_LANES(P, B200_S)
 #undef B200_S
     B200_LAUNCH_CHECK(ctx);
@@ -338,7 +332,8 @@ extern "C" {
     /* elements of `work` (value type): SpMV partials (2k per CTA), then the steps' (2k per CTA) */    \
     int64_t b200_bicgstab_mrhs_work_size_##V(const b200_ctx* ctx, int64_t k)                           \
     {                                                                                                  \
-        return b200::mrhs::spmv_cap(ctx) * 2 * k + b200::mrhs::step_cap(ctx) * 2 * k + 64;             \
+        return b200::mrhs::step_partials_offset<b200::mrhs::DotW2>(ctx, k) +                           \
+               b200::mrhs::step_cap(ctx) * 2 * k + 64;                                                 \
     }                                                                                                  \
     b200_status b200_bicgstab_mrhs_init_##V(b200_ctx* ctx, int64_t n, int64_t k, const VT* r, VT* rr,  \
                                             VT* p, VT* v, VT* y, VT* s, VT* t, VT* z, VT* sc,          \

@@ -22,16 +22,14 @@
 // Scalars  sc[8]: 0 rho, 1 prev_rho, 2 pq, 3 rr, 4 tau0 (baseline norm),
 //                 5 threshold = reduction_factor * tau0, 6/7 local partial sums
 //                 (multi-GPU: all-reduced between step_xr and finish)
-// Control  ctl[8] (int32): 0 stopping_status byte (0 = running), 1 iterations done,
-//                 2 max_iters (-1 none), 3 res_kind (0 none, 1 ResidualNorm,
-//                 2 ImplicitResidualNorm), 4 iter_first
+// Control  ctl[0..4] of fused_common.cuh; 5..7 unused
 #include "csr_launch.cuh"
 #include "fused_common.cuh"
 
 namespace b200 {
 namespace fcg {
 
-using namespace fused;  // kThreads, finish_scalars, ew_grid
+using namespace fused;  // kThreads, grid_sums, finish_scalars, set_threshold, ew_grid
 
 template <typename V>
 __global__ void __launch_bounds__(kThreads)
@@ -64,7 +62,7 @@ __global__ void __launch_bounds__(kThreads)
     const V pq = sc[2];
     const bool update = !INIT && pq != V(0);
     const V alpha = update ? sc[0] / pq : V(0);
-    V a_rho = V(0), a_rr = V(0);
+    V a[2] = {V(0), V(0)};  // rho = r.z, rr = r.r
     for (int64_t i = blockIdx.x * (int64_t)kThreads + tid; i < n;
          i += (int64_t)gridDim.x * kThreads) {
         V ri = r[i];
@@ -75,41 +73,17 @@ __global__ void __launch_bounds__(kThreads)
         }
         const V zi = inv_diag ? ri * inv_diag[i] : ri;
         z[i] = zi;
-        a_rho += ri * zi;
-        a_rr += ri * ri;
+        a[0] += ri * zi;
+        a[1] += ri * ri;
     }
-    a_rho = block_sum(a_rho, red);
-    a_rr = block_sum(a_rr, red);
+    if (!grid_sums(a, partials, counter, red, &is_last)) return;
     if (tid == 0) {
-        partials[2 * blockIdx.x] = a_rho;
-        partials[2 * blockIdx.x + 1] = a_rr;
-        __threadfence();
-        const unsigned int ticket = atomicAdd(counter, 1u);
-        is_last = (ticket == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!is_last) return;
-    __threadfence();
-    V s_rho = V(0), s_rr = V(0);
-    for (int k = tid; k < (int)gridDim.x; k += kThreads) {
-        s_rho += __ldcg(partials + 2 * k);
-        s_rr += __ldcg(partials + 2 * k + 1);
-    }
-    s_rho = block_sum(s_rho, red);
-    s_rr = block_sum(s_rr, red);
-    if (tid == 0) {
-        *counter = 0u;
         if (!finalize) {
-            sc[6] = s_rho;
-            sc[7] = s_rr;
+            sc[6] = a[0];
+            sc[7] = a[1];
         } else {
-            if (INIT) {
-                // baseline: 0 rhs_norm (sc[4] preset to ||b||), 1 initial_resnorm, 2 absolute
-                if (baseline == 1) sc[4] = sqrt(s_rr);
-                if (baseline == 2) sc[4] = V(1);
-                sc[5] = factor * sc[4];
-            }
-            finish_scalars(s_rho, s_rr, sc, ctl);
+            if (INIT) set_threshold(baseline, sqrt(a[1]), sc + 4, sc + 5, factor);
+            finish_scalars(a[0], a[1], sc, ctl);
         }
     }
 }
@@ -122,10 +96,8 @@ __global__ void finish_kernel(V* sc, int32_t* ctl, int baseline, V factor)
     if (INIT) {
         // baseline: 1 initial_resnorm, 2 absolute, 3 rhs_norm with sc[4] = global ||b||^2,
         // 0 rhs_norm with sc[4] = ||b|| already
-        if (baseline == 1) sc[4] = sqrt(sc[7]);
-        if (baseline == 2) sc[4] = V(1);
         if (baseline == 3) sc[4] = sqrt(sc[4]);
-        sc[5] = factor * sc[4];
+        set_threshold(baseline, sqrt(sc[7]), sc + 4, sc + 5, factor);
     }
     finish_scalars(sc[6], sc[7], sc, ctl);
 }
@@ -140,19 +112,7 @@ __global__ void init_scalars_kernel(V* sc, int32_t* ctl, int32_t max_iters, int3
     sc[3] = V(0);
     sc[6] = V(0);
     sc[7] = V(0);
-    ctl[0] = 0;
-    ctl[1] = -1;  // the INIT finish increments to 0
-    ctl[2] = max_iters;
-    ctl[3] = res_kind;
-    ctl[4] = iter_first;
-}
-
-// spmv_dot on a matrix without rows: there are no tiles, so no SpMV kernel runs and writes the dot
-template <typename V>
-__global__ void empty_dot_kernel(V* dot_out, const int32_t* ctl)
-{
-    if (ctl && ctl[0] != 0) return;
-    *dot_out = V(0);
+    start_control(ctl, max_iters, res_kind, iter_first, -1);  // the INIT finish counts to 0
 }
 
 }  // namespace fcg
@@ -209,7 +169,7 @@ void b200_graph_destroy(b200_graph* graph)
     /* elements of `work` (value type) the fused kernels need for a matrix of this size */       \
     int64_t b200_cg_fused_work_size_##V(const b200_ctx* ctx)                                     \
     {                                                                                            \
-        return (int64_t)ctx->num_sms * 4 + 2 * (int64_t)ctx->num_sms * 4 + 64;                   \
+        return b200::fused::work_size(ctx);                                                      \
     }                                                                                            \
     b200_status b200_cg_fused_init_##V(                                                          \
         b200_ctx* ctx, int64_t n, const VT* r, VT* z, VT* p, VT* q, const VT* inv_diag, VT* sc,  \
@@ -218,16 +178,15 @@ void b200_graph_destroy(b200_graph* graph)
     {                                                                                            \
         B200_REQUIRE(ctx && sc && ctl && work, "null argument");                                 \
         b200::fcg::init_scalars_kernel<VT><<<1, 1, 0, ctx->stream>>>(                            \
-            sc, ctl, (int32_t)(max_iters > 0x7fffffff ? 0x7fffffff : max_iters), res_kind,       \
-            iter_first);                                                                         \
+            sc, ctl, b200::fused::clamp_iters(max_iters), res_kind, iter_first);                 \
         B200_LAUNCH_CHECK(ctx);                                                                  \
         B200_CUDA_CHECK(cudaMemsetAsync(p, 0, sizeof(VT) * n, ctx->stream));                     \
         B200_CUDA_CHECK(cudaMemsetAsync(q, 0, sizeof(VT) * n, ctx->stream));                     \
         const int grid = b200::fcg::ew_grid(ctx, n);                                             \
         b200::fcg::step_xr_kernel<VT, true><<<grid, b200::fcg::kThreads, 0, ctx->stream>>>(      \
             n, nullptr, const_cast<VT*>(r), p, q, z, inv_diag, sc, ctl,                          \
-            work + (int64_t)ctx->num_sms * 4, ctx->counters + 2, finalize, baseline,             \
-            reduction_factor);                                                                   \
+            b200::fused::step_partials(ctx, work), ctx->counters + b200::kStepCounter, finalize, \
+            baseline, reduction_factor);                                                         \
         B200_LAUNCH_CHECK(ctx);                                                                  \
         return B200_OK;                                                                          \
     }                                                                                            \
@@ -246,8 +205,8 @@ void b200_graph_destroy(b200_graph* graph)
     {                                                                                            \
         const int grid = b200::fcg::ew_grid(ctx, n);                                             \
         b200::fcg::step_xr_kernel<VT, false><<<grid, b200::fcg::kThreads, 0, ctx->stream>>>(     \
-            n, x, r, p, q, z, inv_diag, sc, ctl, work + (int64_t)ctx->num_sms * 4,               \
-            ctx->counters + 2, finalize, 0, VT(0));                                              \
+            n, x, r, p, q, z, inv_diag, sc, ctl, b200::fused::step_partials(ctx, work),          \
+            ctx->counters + b200::kStepCounter, finalize, 0, VT(0));                             \
         B200_LAUNCH_CHECK(ctx);                                                                  \
         return B200_OK;                                                                          \
     }                                                                                            \
@@ -276,18 +235,9 @@ B200_DEF_FCG(f32, float)
         int64_t nnz, const IT* row_ptrs, const IT* col_idxs, const VT* values, const VT* b,      \
         VT* c, VT* dot_out, VT* work, const int32_t* ctl)                                        \
     {                                                                                            \
-        B200_REQUIRE(ctx && plan && dot_out && work, "null argument (a plan is required)");      \
-        B200_REQUIRE(plan->num_rows == num_rows && plan->nnz == nnz, "plan does not match");     \
-        const b200::csr::Variant v = b200::csr::pick_variant(col_idxs, values, plan);            \
-        B200_REQUIRE(v != b200::csr::kSlab, "col_idxs/values must be 32-byte aligned");          \
-        if (num_rows == 0) {                                                                     \
-            b200::fcg::empty_dot_kernel<VT><<<1, 1, 0, ctx->stream>>>(dot_out, ctl);             \
-            B200_LAUNCH_CHECK(ctx);                                                              \
-            return B200_OK;                                                                      \
-        }                                                                                        \
-        b200::csr::DotArgs<VT> dot{work, ctx->counters + 1, dot_out, ctl};                       \
-        return b200::csr::launch_planned<VT, IT, false, b200::csr::kDotB>(                       \
-            ctx, plan, v, nnz, row_ptrs, col_idxs, values, nullptr, b, 1, nullptr, c, 1, dot);   \
+        return b200::csr::launch_spmv_dot<VT, IT, false, b200::csr::kDotB>(                      \
+            ctx, plan, num_rows, nnz, row_ptrs, col_idxs, values, nullptr, b, nullptr, c,        \
+            nullptr, dot_out, nullptr, work, ctl);                                               \
     }
 
 B200_DEF_SPMV_DOT(f64, double, i32, int32_t)

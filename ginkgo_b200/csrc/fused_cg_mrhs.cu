@@ -21,11 +21,7 @@
 // Scalars  sc[6k]:  sc[s*k + j] for column j, s = 0 rho, 1 prev_rho, 2 pq, 3 rr, 4 tau0 (baseline
 //                   norm), 5 threshold = reduction_factor * tau0
 // Status   status[k]: the reference's stopping_status byte of every column (0 = running)
-// Control  ctl[8] (int32): 0 nonzero once EVERY column has stopped, 1 iterations done, 2 max_iters
-//                   (-1 none), 3 res_kind (0 none, 1 ResidualNorm, 2 ImplicitResidualNorm),
-//                   4 iter_first
-// Once ctl[0] != 0 every kernel is a no-op, so a graph of several iterations can be replayed past
-// the stop.
+// Control  ctl[0..4] of fused_common.cuh; 5..7 unused
 #include "fused_mrhs.cuh"
 
 namespace b200 {
@@ -91,36 +87,16 @@ __global__ void __launch_bounds__(kThreads)
     cta_column_sums<V, P, 2, kThreads>(a, red);
     if (!grid_column_sums<V, 2, kThreads>(a, k, partials, counter, tot, &is_last)) return;
     if (threadIdx.x != 0) return;
-    // the top-of-iteration check of every running column (fused::finish_scalars per column)
+    // the top-of-iteration check of every running column
     const int32_t iter = ctl[1] + 1;
     ctl[1] = iter;
-    bool all_stopped = true;
     for (int c = 0; c < (int)k; ++c) {
-        uint8_t s = status[c];
-        if (!has_stopped(s)) {
-            const V rho_new = tot[0][c], rr = tot[1][c];
-            if (INIT) {
-                // baseline: 0 rhs_norm (sc[4k + c] preset to ||b_c||), 1 initial_resnorm, 2 absolute
-                if (baseline == 1) sc[4 * k + c] = sqrt(rr);
-                if (baseline == 2) sc[4 * k + c] = V(1);
-                sc[5 * k + c] = factor * sc[4 * k + c];
-            }
-            sc[k + c] = sc[c];
-            sc[c] = rho_new;
-            sc[3 * k + c] = rr;
-            const V threshold = sc[5 * k + c];
-            s = fused::criteria_status(
-                iter, ctl,
-                [&](int32_t res_kind) {
-                    const V tau = res_kind == 1 ? sqrt(rr) : sqrt(fabs(rho_new));
-                    return tau <= threshold;
-                },
-                kFinalizedMask);
-            status[c] = s;
-        }
-        all_stopped = all_stopped && has_stopped(s);
+        if (has_stopped(status[c])) continue;
+        const V rr = tot[1][c];
+        if (INIT) fused::set_threshold(baseline, sqrt(rr), sc + 4 * k + c, sc + 5 * k + c, factor);
+        status[c] = fused::top_check(iter, ctl, tot[0][c], rr, sc, k, c);
     }
-    ctl[0] = all_stopped ? 1 : 0;
+    if (all_stopped(k, status)) ctl[0] = 1;
 }
 
 template <typename V>
@@ -135,13 +111,7 @@ __global__ void init_scalars_kernel(int64_t k, V* sc, uint8_t* status, int32_t* 
         sc[3 * k + j] = V(0);
         status[j] = 0;
     }
-    if (j == 0) {
-        ctl[0] = 0;
-        ctl[1] = -1;  // the INIT check increments to 0
-        ctl[2] = max_iters;
-        ctl[3] = res_kind;
-        ctl[4] = iter_first;
-    }
+    if (j == 0) fused::start_control(ctl, max_iters, res_kind, iter_first, -1);  // the INIT check counts to 0
 }
 
 // ---- host side of the entry points ----------------------------------------------------------------
@@ -151,11 +121,12 @@ b200_status step_xr(b200_ctx* ctx, int64_t n, int64_t k, V* x, V* r, const V* p,
 {
     const int P = lanes_for(k);
     const int grid = rows_grid<kThreads>(n, P, step_cap(ctx));
-    V* partials = work + spmv_cap(ctx) * k;
+    V* partials = work + step_partials_offset<DotB>(ctx, k);
 #define B200_XR(PP)                                                                                   \
     step_xr_kernel<V, PP, INIT><<<grid, kThreads, 0, ctx->stream>>>(n, k, x, r, p, q, z, inv_diag, sc, \
                                                                     status, ctl, partials,            \
-                                                                    ctx->counters + 2, baseline, factor)
+                                                                    ctx->counters + kStepCounter,     \
+                                                                    baseline, factor)
     B200_MRHS_BY_LANES(P, B200_XR)
 #undef B200_XR
     B200_LAUNCH_CHECK(ctx);
@@ -169,8 +140,8 @@ b200_status init(b200_ctx* ctx, int64_t n, int64_t k, const V* r, V* z, V* p, V*
 {
     B200_REQUIRE(ctx && sc && status && ctl && work, "null argument");
     B200_REQUIRE(n >= 0 && k >= 2 && k <= kMaxCols, "k must be in [2, 32]");
-    init_scalars_kernel<V><<<1, kMaxCols, 0, ctx->stream>>>(
-        k, sc, status, ctl, (int32_t)(max_iters > 0x7fffffff ? 0x7fffffff : max_iters), res_kind, iter_first);
+    init_scalars_kernel<V><<<1, kMaxCols, 0, ctx->stream>>>(k, sc, status, ctl, fused::clamp_iters(max_iters),
+                                                           res_kind, iter_first);
     B200_LAUNCH_CHECK(ctx);
     if (n > 0) {
         B200_CUDA_CHECK(cudaMemsetAsync(p, 0, sizeof(V) * n * k, ctx->stream));
@@ -204,7 +175,8 @@ extern "C" {
     /* elements of `work` (value type): SpMV partials (k per CTA), then step_xr's (2k per CTA) */     \
     int64_t b200_cg_mrhs_work_size_##V(const b200_ctx* ctx, int64_t k)                               \
     {                                                                                                \
-        return b200::fcgm::spmv_cap(ctx) * k + b200::fcgm::step_cap(ctx) * 2 * k + 64;               \
+        return b200::mrhs::step_partials_offset<b200::mrhs::DotB>(ctx, k) +                         \
+               b200::mrhs::step_cap(ctx) * 2 * k + 64;                                               \
     }                                                                                                \
     b200_status b200_cg_mrhs_init_##V(b200_ctx* ctx, int64_t n, int64_t k, const VT* r, VT* z, VT* p, \
                                       VT* q, const VT* inv_diag, VT* sc, uint8_t* status, int32_t* ctl, \

@@ -33,8 +33,7 @@
 //
 // Scalars  sc[8]:  0 ||w|| of the last final pass (the divisor of the next scale), 1 tau0 (baseline
 //                  norm), 2 threshold = reduction_factor * tau0
-// Control  ctl[8] (int32): 0 stopping_status byte (0 = running), 1 iterations done, 2 max_iters
-//                  (-1 none), 3 res_kind (0 none, 1 ResidualNorm), 4 iter_first
+// Control  ctl[0..4] of fused_common.cuh (res_kind 0 or 1); 5..7 unused, cleared by init
 #include "csr_launch.cuh"
 #include "fused_common.cuh"
 #include "gmres_common.cuh"
@@ -42,7 +41,7 @@
 namespace b200 {
 namespace fgmres {
 
-using namespace fused;  // kThreads, grid_sums, ew_grid
+using namespace fused;  // kThreads, criteria_status, start_control, grid_sums, ew_grid
 
 // the criteria of fused_common.cuh on the GMRES residual estimate tau, by ONE thread, WITHOUT the
 // finalized bit (core/solver/gmres.cpp:453 checks with set_finalized = false)
@@ -64,15 +63,9 @@ template <typename V>
 __global__ void init_kernel(const V* rnorm, V* sc, int32_t* ctl, uint8_t* stop, int32_t max_iters,
                             int32_t res_kind, int32_t iter_first, int32_t baseline, V factor)
 {
-    if (baseline == 1) sc[1] = rnorm[0];
-    if (baseline == 2) sc[1] = V(1);
-    sc[2] = factor * sc[1];
+    set_threshold(baseline, rnorm[0], sc + 1, sc + 2, factor);
     sc[0] = V(0);
-    ctl[0] = 0;
-    ctl[1] = -1;  // the check increments to 0
-    ctl[2] = max_iters;
-    ctl[3] = res_kind;
-    ctl[4] = iter_first;
+    start_control(ctl, max_iters, res_kind, iter_first, -1);  // the check counts to 0
     ctl[5] = ctl[6] = ctl[7] = 0;
     stop[0] = 0;
     check(rnorm[0], sc, ctl, stop);
@@ -172,8 +165,8 @@ extern "C" {
     {                                                                                             \
         B200_REQUIRE(ctx && rnorm && sc && ctl && stop, "null argument");                         \
         b200::fgmres::init_kernel<VT><<<1, 1, 0, ctx->stream>>>(                                  \
-            rnorm, sc, ctl, stop, (int32_t)(max_iters > 0x7fffffff ? 0x7fffffff : max_iters),     \
-            res_kind, iter_first, baseline, reduction_factor);                                    \
+            rnorm, sc, ctl, stop, b200::fused::clamp_iters(max_iters), res_kind, iter_first,      \
+            baseline, reduction_factor);                                                          \
         B200_LAUNCH_CHECK(ctx);                                                                   \
         return B200_OK;                                                                           \
     }                                                                                             \
@@ -196,8 +189,8 @@ extern "C" {
         B200_REQUIRE(i >= 1, "pass index must be >= 1");                                          \
         const int grid = b200::fused::ew_grid(ctx, n);                                            \
         b200::fgmres::mgs_pass_kernel<VT><<<grid, b200::fused::kThreads, 0, ctx->stream>>>(       \
-            n, w, v_prev, v_i, hcol, i, ctl, work + (int64_t)ctx->num_sms * 4,                    \
-            ctx->counters + 2);                                                                   \
+            n, w, v_prev, v_i, hcol, i, ctl, b200::fused::step_partials(ctx, work),               \
+            ctx->counters + b200::kStepCounter);                                                  \
         B200_LAUNCH_CHECK(ctx);                                                                   \
         return B200_OK;                                                                           \
     }                                                                                             \
@@ -225,7 +218,7 @@ extern "C" {
         const int grid = b200::fused::ew_grid(ctx, n);                                            \
         b200::fgmres::sub_pass_kernel<VT, true><<<grid, b200::fused::kThreads, 0, ctx->stream>>>( \
             n, w, krylov, first, coef, haux, hcol, j, gsin, gcos, rnorm, rnc, fin, stop, sc, ctl, \
-            work + (int64_t)ctx->num_sms * 4, ctx->counters + 2);                                 \
+            b200::fused::step_partials(ctx, work), ctx->counters + b200::kStepCounter);           \
         B200_LAUNCH_CHECK(ctx);                                                                   \
         return B200_OK;                                                                           \
     }

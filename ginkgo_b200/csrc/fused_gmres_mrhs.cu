@@ -36,8 +36,7 @@
 // Scalars  sc[3k]: sc[s*k + c], s = 0 ||w|| of the last final pass (the divisor of the next scale),
 //                  1 tau0 (baseline norm), 2 threshold = reduction_factor * tau0
 // Status   status[k]: the loop's stopping_status byte of every column (0 = running)
-// Control  ctl[8] (int32): 0 nonzero once EVERY column has stopped, 1 iterations done, 2 max_iters
-//                  (-1 none), 3 res_kind (0 none, 1 ResidualNorm), 4 iter_first
+// Control  ctl[0..4] of fused_common.cuh (res_kind 0 or 1); 5..7 unused, cleared by init
 #include "fused_mrhs.cuh"
 #include "gmres_common.cuh"
 
@@ -51,9 +50,11 @@ constexpr int kMdThreads = 256;
 constexpr int kMdBases = 16;  // bases per sweep of the multi-dot (register accumulators)
 
 inline int64_t md_cap(const b200_ctx* ctx) { return (int64_t)ctx->num_sms * kStepCtasPerSm; }
-// `work`: the SpMV's partials (2k per CTA), the passes' (k per CTA), the multi-dot's ((kd+1) k per CTA)
-inline int64_t pass_offset(const b200_ctx* ctx, int64_t k) { return spmv_cap(ctx) * 2 * k; }
-inline int64_t md_offset(const b200_ctx* ctx, int64_t k) { return pass_offset(ctx, k) + step_cap(ctx) * k; }
+// `work`: the SpMV's partials (DotW2), the passes' (k per CTA), the multi-dot's ((kd+1) k per CTA)
+inline int64_t md_offset(const b200_ctx* ctx, int64_t k)
+{
+    return step_partials_offset<DotW2>(ctx, k) + step_cap(ctx) * k;
+}
 inline int64_t work_size(const b200_ctx* ctx, int64_t k, int64_t krylov_dim)
 {
     return md_offset(ctx, k) + md_cap(ctx) * (krylov_dim + 1) * k + 64;
@@ -65,14 +66,6 @@ __device__ __forceinline__ uint8_t column_status(int32_t iter, const int32_t* ct
     return fused::criteria_status(iter, ctl, [&](int32_t) { return tau <= threshold; }, uint8_t(0));
 }
 
-// thread 0, after every column's status is written: ctl[0] once all columns have stopped
-__device__ __forceinline__ void raise_if_all_stopped(int64_t k, const uint8_t* status, int32_t* ctl)
-{
-    bool all_stopped = true;
-    for (int c = 0; c < (int)k; ++c) all_stopped = all_stopped && has_stopped(status[c]);
-    if (all_stopped) ctl[0] = 1;
-}
-
 // rnorm holds ||b_c - A x_c|| (the loop's norm2); v_0, rnc, fin, gsin and gcos are set by the loop's
 // initialize / restart kernels; sc[k + c] holds ||b_c|| for the rhs_norm baseline
 template <typename V>
@@ -81,24 +74,17 @@ __global__ void init_kernel(int64_t k, const V* rnorm, V* sc, uint8_t* status, i
 {
     const int c = threadIdx.x;
     if (c == 0) {
-        ctl[0] = 0;
-        ctl[1] = 0;
-        ctl[2] = max_iters;
-        ctl[3] = res_kind;
-        ctl[4] = iter_first;
+        fused::start_control(ctl, max_iters, res_kind, iter_first, 0);
         ctl[5] = ctl[6] = ctl[7] = 0;
     }
     __syncthreads();
     if (c < k) {
-        if (baseline == 1) sc[k + c] = rnorm[c];
-        if (baseline == 2) sc[k + c] = V(1);
-        const V threshold = factor * sc[k + c];
-        sc[2 * k + c] = threshold;
+        fused::set_threshold(baseline, rnorm[c], sc + k + c, sc + 2 * k + c, factor);
         sc[c] = V(0);
-        status[c] = column_status(0, ctl, rnorm[c], threshold);
+        status[c] = column_status(0, ctl, rnorm[c], sc[2 * k + c]);
     }
     __syncthreads();
-    if (c == 0) raise_if_all_stopped(k, status, ctl);
+    if (c == 0 && all_stopped(k, status)) ctl[0] = 1;
 }
 
 template <typename V, int P>
@@ -206,7 +192,7 @@ __global__ void __launch_bounds__(kThreads)
     __syncthreads();
     if (c == 0) {
         ctl[1] = iter;
-        raise_if_all_stopped(k, status, ctl);
+        if (all_stopped(k, status)) ctl[0] = 1;
     }
 }
 
@@ -250,24 +236,9 @@ __global__ void __launch_bounds__(kMdThreads, 2)
                 if (q < nb) partials[blockIdx.x * per_cta + (i0 + q) * k + tid] = acc[q];
     }
     if (tid < k) __threadfence();
-    __syncthreads();
-    if (tid == 0) {
-        const unsigned int ticket = atomicAdd(counter, 1u);
-        is_last = (ticket == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!is_last) return;
-    __threadfence();
-    const int lane = tid & 31, warp = tid >> 5;
-    for (int64_t idx = warp; idx < per_cta; idx += kMdThreads / 32) {
-        V s = V(0);
-        for (int c = lane; c < (int)gridDim.x; c += 32) s += __ldcg(partials + c * per_cta + idx);
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-        if (lane == 0 && !has_stopped(status[idx % k])) hcol[idx] = s;
-    }
-    __syncthreads();
-    if (tid == 0) *counter = 0u;
+    last_cta_sums<kMdThreads>(per_cta, partials, counter, &is_last, [&](int64_t idx, V s) {
+        if (!has_stopped(status[idx % k])) hcol[idx] = s;  // a stopped column keeps its Hessenberg entries
+    });
 }
 
 // ---- host side of the entry points ----------------------------------------------------------------
@@ -282,8 +253,8 @@ b200_status init(b200_ctx* ctx, int64_t k, const V* rnorm, V* sc, uint8_t* statu
     B200_FGM_REQUIRE(ctx, 0, k);
     B200_REQUIRE(rnorm && sc && status && ctl, "null argument");
     init_kernel<V><<<1, kMaxCols, 0, ctx->stream>>>(k, rnorm, sc, status, ctl,
-                                                   (int32_t)(max_iters > 0x7fffffff ? 0x7fffffff : max_iters),
-                                                   res_kind, iter_first, baseline, factor);
+                                                   fused::clamp_iters(max_iters), res_kind, iter_first, baseline,
+                                                   factor);
     B200_LAUNCH_CHECK(ctx);
     return B200_OK;
 }
@@ -313,10 +284,10 @@ b200_status mgs_pass(b200_ctx* ctx, int64_t n, int64_t k, V* w, const V* v_prev,
     B200_REQUIRE(i >= 1, "pass index must be >= 1");
     const int P = lanes_for(k);
     const int grid = rows_grid<kThreads>(n, P, step_cap(ctx));
-    V* partials = work + pass_offset(ctx, k);
+    V* partials = work + step_partials_offset<DotW2>(ctx, k);
 #define B200_MG(PP)                                                                                      \
     mgs_pass_kernel<V, PP><<<grid, kThreads, 0, ctx->stream>>>(n, k, w, v_prev, v_i, hcol, i, status, ctl, \
-                                                               partials, ctx->counters + 2)
+                                                               partials, ctx->counters + kStepCounter)
     B200_MRHS_BY_LANES(P, B200_MG)
 #undef B200_MG
     B200_LAUNCH_CHECK(ctx);
@@ -333,12 +304,12 @@ b200_status sub_pass(b200_ctx* ctx, int64_t n, int64_t k, V* w, const V* krylov,
     B200_REQUIRE(j >= 0 && first >= 0 && first <= j, "need 0 <= first <= j");
     const int P = lanes_for(k);
     const int grid = rows_grid<kThreads>(n, P, step_cap(ctx));
-    V* partials = FINAL ? work + pass_offset(ctx, k) : nullptr;
+    V* partials = FINAL ? work + step_partials_offset<DotW2>(ctx, k) : nullptr;
 #define B200_SP(PP)                                                                                       \
     sub_pass_kernel<V, PP, FINAL><<<grid, kThreads, 0, ctx->stream>>>(n, k, w, krylov, first, coef, haux, \
                                                                       hcol, j, gsin, gcos, rnorm, rnc, fin, \
                                                                       status, sc, ctl, partials,          \
-                                                                      ctx->counters + 2)
+                                                                      ctx->counters + kStepCounter)
     B200_MRHS_BY_LANES(P, B200_SP)
 #undef B200_SP
     B200_LAUNCH_CHECK(ctx);
@@ -358,7 +329,7 @@ b200_status multi_dot(b200_ctx* ctx, int64_t n, int64_t k, int64_t num_bases, in
     V* partials = work + md_offset(ctx, k);
 #define B200_MD(PP)                                                                                        \
     multi_dot_kernel<V, PP><<<grid, kMdThreads, 0, ctx->stream>>>(n, k, num_bases, krylov, w, hcol, status, \
-                                                                  ctl, partials, ctx->counters + 3)
+                                                                  ctl, partials, ctx->counters + kMultiDotCounter)
     B200_MRHS_BY_LANES(P, B200_MD)
 #undef B200_MD
     B200_LAUNCH_CHECK(ctx);

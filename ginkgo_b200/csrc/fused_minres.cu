@@ -31,15 +31,14 @@
 // Scalars  sc[16]: 0 alpha, 1 beta, 2 gamma, 3 delta, 4 tau0 (baseline norm), 5 threshold =
 //                  reduction_factor * tau0, 6 tau, 7 eta, 8 eta_next, 9 cos_prev, 10 cos, 11 sin_prev,
 //                  12 sin
-// Control  ctl[8] (int32): 0 stopping_status byte (0 = running), 1 iterations done, 2 max_iters
-//                  (-1 none), 3 res_kind (0 none, 2 ImplicitResidualNorm), 4 iter_first
+// Control  ctl[0..4] of fused_common.cuh (res_kind 0 or 2); 5..7 unused, cleared by init
 #include "csr_launch.cuh"
 #include "fused_common.cuh"
 
 namespace b200 {
 namespace fminres {
 
-using namespace fused;  // kThreads, grid_sums, criteria_status, ew_grid
+using namespace fused;  // kThreads, grid_sums, last_ticket, criteria_status, set_threshold, ew_grid
 
 // include/ginkgo/core/base/math.hpp, as krylov_steps.cu states them
 template <typename V>
@@ -158,13 +157,8 @@ __global__ void __launch_bounds__(kThreads)
     }
     // the ticket of fused::grid_sums without the sums: every CTA has read ctl[1] and the scalars
     __syncthreads();
-    if (tid == 0) {
-        __threadfence();
-        const unsigned int ticket = atomicAdd(counter, 1u);
-        is_last = (ticket == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!is_last || tid != 0) return;
+    if (tid == 0) __threadfence();
+    if (!last_ticket(counter, &is_last) || tid != 0) return;
     *counter = 0u;
     // std::swap(gamma, beta) of the loop, by value
     sc[1] = gamma;
@@ -181,24 +175,12 @@ template <typename V>
 __global__ void init_kernel(V* sc, int32_t* ctl, int32_t max_iters, int32_t res_kind, int32_t iter_first,
                             int32_t baseline, V factor)
 {
-    if (baseline == 2) sc[4] = V(1);
-    sc[5] = factor * sc[4];
-    ctl[1] = 0;
-    ctl[2] = max_iters;
-    ctl[3] = res_kind;
-    ctl[4] = iter_first;
+    set_threshold(baseline, sc[4], sc + 4, sc + 5, factor);  // baseline 1: the host put ||r0|| in sc[4]
+    start_control(ctl, max_iters, res_kind, iter_first, 0);
     ctl[5] = ctl[6] = ctl[7] = 0;
     const V tau = sc[6];
     ctl[0] = criteria_status(
         0, ctl, [&](int32_t) { return sqrt(fabs(tau)) <= sc[5]; }, kFinalizedMask);
-}
-
-// spmv_sub_dot on a matrix without rows: there are no tiles, so no SpMV kernel runs and writes the dot
-template <typename V>
-__global__ void empty_dot_kernel(V* dot_out, const int32_t* ctl)
-{
-    if (ctl && ctl[0] != 0) return;
-    *dot_out = V(0);
 }
 
 // the (alpha, beta) = (1, -1) of the advanced SpMV, as device scalars
@@ -214,7 +196,7 @@ extern "C" {
     /* elements of `work` (value type) the fused kernels need */                                  \
     int64_t b200_minres_fused_work_size_##V(const b200_ctx* ctx)                                  \
     {                                                                                             \
-        return (int64_t)ctx->num_sms * 4 + 2 * (int64_t)ctx->num_sms * 4 + 64;                    \
+        return b200::fused::work_size(ctx);                                                       \
     }                                                                                             \
     b200_status b200_minres_fused_init_##V(b200_ctx* ctx, VT* sc, int32_t* ctl, int64_t max_iters, \
                                            int32_t res_kind, int32_t iter_first, int32_t baseline, \
@@ -222,8 +204,8 @@ extern "C" {
     {                                                                                             \
         B200_REQUIRE(ctx && sc && ctl, "null argument");                                          \
         b200::fminres::init_kernel<VT><<<1, 1, 0, ctx->stream>>>(                                 \
-            sc, ctl, (int32_t)(max_iters > 0x7fffffff ? 0x7fffffff : max_iters), res_kind,        \
-            iter_first, baseline, reduction_factor);                                              \
+            sc, ctl, b200::fused::clamp_iters(max_iters), res_kind, iter_first, baseline,         \
+            reduction_factor);                                                                    \
         B200_LAUNCH_CHECK(ctx);                                                                   \
         return B200_OK;                                                                           \
     }                                                                                             \
@@ -234,7 +216,8 @@ extern "C" {
         B200_REQUIRE(ctx && sc && ctl && work, "null argument");                                  \
         const int grid = b200::fused::ew_grid(ctx, n);                                            \
         b200::fminres::lanczos_kernel<VT><<<grid, b200::fused::kThreads, 0, ctx->stream>>>(       \
-            n, v, q, inv_diag, sc, ctl, work + (int64_t)ctx->num_sms * 4, ctx->counters + 2);     \
+            n, v, q, inv_diag, sc, ctl, b200::fused::step_partials(ctx, work),                    \
+            ctx->counters + b200::kStepCounter);                                                  \
         B200_LAUNCH_CHECK(ctx);                                                                   \
         return B200_OK;                                                                           \
     }                                                                                             \
@@ -245,7 +228,7 @@ extern "C" {
         B200_REQUIRE(ctx && sc && ctl, "null argument");                                          \
         const int grid = b200::fused::ew_grid(ctx, n);                                            \
         b200::fminres::update_kernel<VT><<<grid, b200::fused::kThreads, 0, ctx->stream>>>(        \
-            n, x, p0, p1, z, q, v, inv_diag, sc, ctl, ctx->counters + 2);                         \
+            n, x, p0, p1, z, q, v, inv_diag, sc, ctl, ctx->counters + b200::kStepCounter);        \
         B200_LAUNCH_CHECK(ctx);                                                                   \
         return B200_OK;                                                                           \
     }
@@ -261,20 +244,11 @@ B200_DEF_FMINRES(f32, float)
         int64_t nnz, const IT* row_ptrs, const IT* col_idxs, const VT* values, const VT* b,       \
         VT* c, VT* dot_out, VT* work, const int32_t* ctl)                                         \
     {                                                                                             \
-        B200_REQUIRE(ctx && plan && dot_out && work, "null argument (a plan is required)");       \
-        B200_REQUIRE(plan->num_rows == num_rows && plan->nnz == nnz, "plan does not match");      \
-        const b200::csr::Variant v = b200::csr::pick_variant(col_idxs, values, plan);             \
-        B200_REQUIRE(v != b200::csr::kSlab, "col_idxs/values must be 32-byte aligned");           \
-        if (num_rows == 0) {                                                                      \
-            b200::fminres::empty_dot_kernel<VT><<<1, 1, 0, ctx->stream>>>(dot_out, ctl);          \
-            B200_LAUNCH_CHECK(ctx);                                                               \
-            return B200_OK;                                                                       \
-        }                                                                                         \
         VT* ab = nullptr;                                                                         \
         B200_CUDA_CHECK(cudaGetSymbolAddress((void**)&ab, b200::fminres::one_neg_one_##V));       \
-        b200::csr::DotArgs<VT> dot{work, ctx->counters + 1, dot_out, ctl};                        \
-        return b200::csr::launch_planned<VT, IT, true, b200::csr::kDotB>(                         \
-            ctx, plan, v, nnz, row_ptrs, col_idxs, values, ab, b, 1, ab + 1, c, 1, dot);          \
+        return b200::csr::launch_spmv_dot<VT, IT, true, b200::csr::kDotB>(                        \
+            ctx, plan, num_rows, nnz, row_ptrs, col_idxs, values, ab, b, ab + 1, c, nullptr,      \
+            dot_out, nullptr, work, ctl);                                                         \
     }
 
 B200_DEF_SPMV_SUB_DOT(f64, double, i32, int32_t)

@@ -1,6 +1,7 @@
-// What the fused iterations for k = 2..32 right-hand sides (fused_cg_mrhs.cu, fused_bicgstab_mrhs.cu)
-// share: the row / lane layout of their n x k row-major vectors (stride k), the bounded grids, the
-// per-column sums and the SpMV whose epilogue sums per-column products.
+// What the fused iterations for k = 2..32 right-hand sides (fused_cg_mrhs.cu, fused_bicgstab_mrhs.cu,
+// fused_gmres_mrhs.cu) share: the row / lane layout of their n x k row-major vectors (stride k), the
+// bounded grids and the workspace, the per-column sums, the all-stopped test and the SpMV whose epilogue
+// sums per-column products.
 //
 // Layout: P = next power of two >= k lanes per row; lane j works on column j of the k-wide row.
 // Grids are bounded and walk the rows grid-stride, so the per-CTA partials fit a fixed workspace.
@@ -61,39 +62,64 @@ __device__ __forceinline__ void cta_column_sums(V (&a)[NV], V (&red)[NV][THREADS
         }
 }
 
-// the grid-wide part: thread j < k publishes its column's NV CTA sums, and the CTA with the last
-// ticket adds the partials of every (sum, column) in CTA order -- one warp per (sum, column), lanes
-// over the CTAs, then a fixed shuffle tree -- into tot[v][j].  Returns true in that CTA only, after a
+// The last-CTA part of a grid-wide sum of per_cta values per CTA (partials[c * per_cta + idx] from CTA
+// c), by every thread once the CTA's partials are written and fenced: the ticket, then in the CTA with
+// the last one the partials of every index in CTA order -- one warp per index, lanes over the CTAs, then
+// a fixed shuffle tree -- handed to store(idx, sum) by lane 0.  Returns true in that CTA only, after a
 // barrier; the ticket is back at 0.
+template <int THREADS, typename V, typename Store>
+__device__ __forceinline__ bool last_cta_sums(int64_t per_cta, const V* __restrict__ partials,
+                                              unsigned int* counter, bool* is_last, Store store)
+{
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    __syncthreads();
+    if (!fused::last_ticket(counter, is_last)) return false;
+    __threadfence();
+    for (int idx = warp; idx < per_cta; idx += THREADS / 32) {
+        V s = V(0);
+        for (int c = lane; c < (int)gridDim.x; c += 32) s += __ldcg(partials + c * per_cta + idx);
+        s = warp_sum(s);
+        if (lane == 0) store(idx, s);
+    }
+    __syncthreads();
+    if (tid == 0) *counter = 0u;
+    return true;
+}
+
+// the grid-wide part of NV sums per column: thread j < k publishes its column's NV CTA sums, and the CTA
+// with the last ticket adds the partials of every (sum, column) into tot[v][j] (last_cta_sums).  Returns
+// true in that CTA only, after a barrier; the ticket is back at 0.
 template <typename V, int NV, int THREADS>
 __device__ __forceinline__ bool grid_column_sums(const V (&a)[NV], int64_t k, V* __restrict__ partials,
                                                  unsigned int* counter, V (&tot)[NV][kMaxCols], bool* is_last)
 {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const int64_t per_cta = NV * k;
     if (tid < k) {
 #pragma unroll
         for (int v = 0; v < NV; ++v) partials[blockIdx.x * per_cta + v * k + tid] = a[v];
         __threadfence();
     }
-    __syncthreads();
-    if (tid == 0) {
-        const unsigned int ticket = atomicAdd(counter, 1u);
-        *is_last = (ticket == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!*is_last) return false;
-    __threadfence();
-    for (int idx = warp; idx < per_cta; idx += THREADS / 32) {
-        V s = V(0);
-        for (int c = lane; c < (int)gridDim.x; c += 32) s += __ldcg(partials + c * per_cta + idx);
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-        if (lane == 0) tot[idx / k][idx % k] = s;
-    }
-    __syncthreads();
-    if (tid == 0) *counter = 0u;
-    return true;
+    return last_cta_sums<THREADS>(per_cta, partials, counter, is_last,
+                                  [&](int idx, V s) { tot[idx / k][idx % k] = s; });
+}
+
+// By thread 0, after every column's status is written: have all k columns stopped?  The callers raise
+// ctl[0] = 1 then and otherwise leave ctl[0] as it is, which is the same as writing 0: a kernel that gets
+// here started with ctl[0] == 0 (it returns at entry otherwise, and init has just cleared it).
+__device__ __forceinline__ bool all_stopped(int64_t k, const uint8_t* status)
+{
+    bool all = true;
+    for (int c = 0; c < (int)k; ++c) all = all && has_stopped(status[c]);
+    return all;
+}
+
+// `work` of the k-column paths: the SpMV's partials (Epi::NV k per CTA), then the step kernels' from this
+// offset on
+template <typename Epi>
+inline int64_t step_partials_offset(const b200_ctx* ctx, int64_t k)
+{
+    return spmv_cap(ctx) * Epi::NV * k;
 }
 
 // SpMV epilogues: what each (row, column) of c adds to its column's sums, and where the sums go.
@@ -204,9 +230,8 @@ b200_status spmv_mdot(b200_ctx* ctx, int64_t num_rows, int64_t num_cols, int64_t
     const int P = lanes_for(k);
     const int grid = rows_grid<kSpmvThreads>(num_rows, P, spmv_cap(ctx));
 #define B200_MD(PP)                                                                                      \
-    spmv_mdot_kernel<V, I, PP, Epi><<<grid, kSpmvThreads, 0, ctx->stream>>>(num_rows, k, row_ptrs, col_idxs, \
-                                                                            values, b, c, w, dots, dots2,     \
-                                                                            partials, ctx->counters + 1, ctl)
+    spmv_mdot_kernel<V, I, PP, Epi><<<grid, kSpmvThreads, 0, ctx->stream>>>(                              \
+        num_rows, k, row_ptrs, col_idxs, values, b, c, w, dots, dots2, partials, ctx->counters + kSpmvDotCounter, ctl)
     B200_MRHS_BY_LANES(P, B200_MD)
 #undef B200_MD
     B200_LAUNCH_CHECK(ctx);

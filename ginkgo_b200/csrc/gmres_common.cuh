@@ -1,15 +1,17 @@
 // What the GMRES loop kernels (gmres_kernels.cu) and the fused GMRES iteration (fused_gmres.cu) share:
-// the Givens update of one Hessenberg column.
+// the Givens update of one Hessenberg column, and the workspace offset of the fused multi-dot (after the
+// one-column workspace of fused_common.cuh).
 #pragma once
-#include "common.cuh"
+#include "fused_common.cuh"
 
 namespace b200 {
 namespace gmres {
 
-// workspace of the fused iteration (b200_gmres_fused_work_size): per-CTA partials of the SpMV + dot and
-// of the passes (up to 4 CTAs per SM each), then those of the multi-dot, one per CTA and basis
+// workspace of the fused iteration (b200_gmres_fused_work_size): the one-column workspace of
+// fused_common.cuh (the SpMV + dot's and the passes' partials), then those of the multi-dot, one per CTA
+// and basis
 constexpr int kFusedMdCtasPerSm = 4;
-inline int64_t fused_md_offset(const b200_ctx* ctx) { return (int64_t)ctx->num_sms * 12 + 64; }
+inline int64_t fused_md_offset(const b200_ctx* ctx) { return fused::work_size(ctx); }
 inline int64_t fused_work_size(const b200_ctx* ctx, int64_t krylov_dim)
 {
     return fused_md_offset(ctx) + (int64_t)ctx->num_sms * kFusedMdCtasPerSm * (krylov_dim + 1);

@@ -258,10 +258,10 @@ b200_status fused_multi_dot(b200_ctx* ctx, int64_t rows, int64_t num_bases, cons
     V* partials = work + fused_md_offset(ctx);
     if (vec_ok)
         multi_dot_kernel<V, kVW, true><<<grid, kMdThreads, 0, ctx->stream>>>(
-            rows, 1, num_bases, krylov, 1, w, 1, partials, ctx->counters + 3, hcol, 1, ctl);
+            rows, 1, num_bases, krylov, 1, w, 1, partials, ctx->counters + kMultiDotCounter, hcol, 1, ctl);
     else
         multi_dot_kernel<V, 1, true><<<grid, kMdThreads, 0, ctx->stream>>>(
-            rows, 1, num_bases, krylov, 1, w, 1, partials, ctx->counters + 3, hcol, 1, ctl);
+            rows, 1, num_bases, krylov, 1, w, 1, partials, ctx->counters + kMultiDotCounter, hcol, 1, ctl);
     B200_LAUNCH_CHECK(ctx);
     return B200_OK;
 }
