@@ -523,7 +523,10 @@ class HostSolver:
     gaps between columns, Identity or scalar Jacobi, Iteration / ResidualNorm; one matrix pass per SpMV
     for all columns, each column stops on its own; block Jacobi and anything else take the loop);
     fused_minres: Minres's, opt-in (Csr, one right-hand side, Identity or scalar Jacobi, Iteration /
-    ImplicitResidualNorm; three launches per iteration; ResidualNorm and anything else take the loop).
+    ImplicitResidualNorm; three launches per iteration; ResidualNorm and anything else take the loop);
+    fused_minres_multi_rhs: Minres's for 2..32 right-hand sides, opt-in and independent of fused_minres
+    (b and x without gaps between columns, otherwise fused_minres's admission; one matrix pass per
+    iteration for all columns, each column stops on its own).
     check_every: iterations per graph launch on those paths.  preconditioner: a generated one (host_jacobi, e.g. with
     storage_optimization) used in place of precond_max_bs.  used_fused tells after apply whether such a
     path ran; stop_status is column 0's stopping status, stop_statuses every column's."""
@@ -532,7 +535,8 @@ class HostSolver:
                  res_kind=1, baseline=0, reduction=1e-8, iter_first=True, krylov_dim=30, ortho=0,
                  fused=True, check_every=16, relaxation_factor=1.0, foci=(0.0, 1.0), initial_guess="provided",
                  fused_bicgstab=False, fused_gmres=False, preconditioner=None, fused_multi_rhs=False,
-                 fused_bicgstab_multi_rhs=False, fused_gmres_multi_rhs=False, fused_minres=False):
+                 fused_bicgstab_multi_rhs=False, fused_gmres_multi_rhs=False, fused_minres=False,
+                 fused_minres_multi_rhs=False):
         self.vt = A.vt
         _host().gkob_solver_params(float(relaxation_factor), float(foci[0]), float(foci[1]))
         # "ir" only: solver::initial_guess_mode of with_default_initial_guess
@@ -553,7 +557,8 @@ class HostSolver:
                                       (4 if fused_gmres else 0) | (8 if fused_multi_rhs else 0) |
                                       (16 if fused_bicgstab_multi_rhs else 0) |
                                       (32 if fused_gmres_multi_rhs else 0) |
-                                      (64 if fused_minres else 0),
+                                      (64 if fused_minres else 0) |
+                                      (128 if fused_minres_multi_rhs else 0),
                                       check_every), (A,))
 
     def apply(self, b, x):

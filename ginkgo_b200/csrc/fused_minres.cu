@@ -33,71 +33,12 @@
 //                  12 sin
 // Control  ctl[0..4] of fused_common.cuh (res_kind 0 or 2); 5..7 unused, cleared by init
 #include "csr_launch.cuh"
-#include "fused_common.cuh"
+#include "fused_minres.cuh"
 
 namespace b200 {
 namespace fminres {
 
 using namespace fused;  // kThreads, grid_sums, last_ticket, criteria_status, set_threshold, ew_grid
-
-// include/ginkgo/core/base/math.hpp, as krylov_steps.cu states them
-template <typename V>
-__device__ __forceinline__ V safe_divide(V a, V b)
-{
-    return b == V(0) ? V(0) : a / b;
-}
-template <typename V>
-__device__ __forceinline__ V dev_abs(V a)
-{
-    return a < V(0) ? -a : a;
-}
-
-// minres::step_1 (krylov_steps.cu, reference/solver/minres_kernels.cpp:64-110) on the scalar block,
-// by ONE thread, with beta = v.z~ just summed
-template <typename V>
-__device__ void step_1(V beta_sq, V* sc)
-{
-    const V bt = sqrt(beta_sq);
-    sc[1] = bt;
-    const V tmp_d = sc[2];
-    const V tmp_a = sc[0];
-    sc[3] = sc[11] * tmp_d;
-    const V c_old = sc[10], s_old = sc[12], cp_old = sc[9];
-    const V g1 = cp_old * c_old;
-    const V g2 = g1 * tmp_d;
-    const V g3 = s_old * tmp_a;
-    sc[2] = g2 + g3;
-    const V a1 = (-s_old) * cp_old;
-    const V a2 = a1 * tmp_d;
-    const V a3 = c_old * tmp_a;
-    V al = a2 + a3;
-    sc[9] = c_old;
-    sc[11] = s_old;
-    V c, sn;
-    if (al == V(0)) {
-        c = V(0);
-        sn = V(1);
-    } else {
-        const V scale = dev_abs(al) + dev_abs(bt);
-        const V ra = dev_abs(al / scale), rb = dev_abs(bt / scale);
-        const V h1 = ra * ra;
-        const V h2 = rb * rb;
-        const V hyp = scale * sqrt(h1 + h2);
-        c = al / hyp;
-        sn = bt / hyp;
-    }
-    const V n1 = c * al;
-    const V n2 = sn * bt;
-    al = n1 + n2;
-    sc[0] = al;
-    sc[10] = c;
-    sc[12] = sn;
-    const V t1 = sn * sn;
-    sc[6] = t1 * sc[6];
-    const V e = sc[8];
-    sc[7] = e;
-    sc[8] = (-sn) * e;
-}
 
 template <typename V>
 __global__ void __launch_bounds__(kThreads)
@@ -122,7 +63,7 @@ __global__ void __launch_bounds__(kThreads)
     }
     // every CTA read alpha before it took its ticket: the last one may overwrite the scalars
     if (!grid_sums(a, partials, counter, red, &is_last)) return;
-    if (threadIdx.x == 0) step_1(a[0], sc);
+    if (threadIdx.x == 0) step_1(a[0], sc, 1);
 }
 
 template <typename V>

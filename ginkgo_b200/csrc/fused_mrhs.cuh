@@ -1,5 +1,5 @@
 // What the fused iterations for k = 2..32 right-hand sides (fused_cg_mrhs.cu, fused_bicgstab_mrhs.cu,
-// fused_gmres_mrhs.cu) share: the row / lane layout of their n x k row-major vectors (stride k), the
+// fused_gmres_mrhs.cu, fused_minres_mrhs.cu) share: the row / lane layout of their n x k row-major vectors (stride k), the
 // bounded grids and the workspace, the per-column sums, the all-stopped test and the SpMV whose epilogue
 // sums per-column products.
 //
@@ -122,10 +122,12 @@ inline int64_t step_partials_offset(const b200_ctx* ctx, int64_t k)
     return spmv_cap(ctx) * Epi::NV * k;
 }
 
-// SpMV epilogues: what each (row, column) of c adds to its column's sums, and where the sums go.
+// SpMV epilogues: what each (row, column) of c adds to its column's sums, and where the sums go, and
+// SUB: whether the SpMV is c = A b - c (the advanced SpMV with (1, -1)) instead of c = A b.
 // DotB: dots[j] = sum b_j . c_j (b is the SpMV input: CG's p . A p).
 struct DotB {
     static constexpr int NV = 1;
+    static constexpr bool SUB = false;
     template <typename V>
     __device__ __forceinline__ static void add(V (&a)[NV], const V* __restrict__ b, const V* __restrict__ w,
                                                int64_t e, V c)
@@ -142,6 +144,7 @@ struct DotB {
 // dots2 is null (BiCGStab's rr . v, and s . t with t . t)
 struct DotW2 {
     static constexpr int NV = 2;
+    static constexpr bool SUB = false;
     template <typename V>
     __device__ __forceinline__ static void add(V (&a)[NV], const V* __restrict__ b, const V* __restrict__ w,
                                                int64_t e, V c)
@@ -156,10 +159,17 @@ struct DotW2 {
         if (dots2) dots2[j] = tot[1][j];
     }
 };
+// SubDotB: c = A b - c and DotB's sums (MINRES's v = A z - v, alpha = z . v)
+struct SubDotB : DotB {
+    static constexpr bool SUB = true;
+};
 
-// c = A b for k columns (b, c, w: stride k), the epilogue's per-column sums into dots / dots2.  Lane j
-// gathers column j of the k-wide row of b and every (row, column) sum runs left to right: the layout
-// of multi_rhs_rows_kernel (csr_kernels.cuh), so c is bit-identical to b200_csr_spmv_* with num_rhs = k.
+// c = A b (Epi::SUB: A b - c) for k columns (b, c, w: stride k), the epilogue's per-column sums into
+// dots / dots2.  Lane j gathers column j of the k-wide row of b and every (row, column) sum runs left to
+// right: the layout of multi_rhs_rows_kernel (csr_kernels.cuh), so c is bit-identical to b200_csr_spmv_*
+// with num_rhs = k.  SUB seeds each sum with c * (-1) before the products, as that kernel's ADVANCED
+// mode does with (alpha, beta) = (1, -1) (acc = c beta; acc += (alpha v) x, and 1 * v is exact): c is
+// bit-identical to b200_csr_advanced_spmv_* with (1, -1) and num_rhs = k.
 template <typename V, typename I, int P, typename Epi>
 __global__ void __launch_bounds__(kSpmvThreads)
     spmv_mdot_kernel(int64_t num_rows, int64_t k, const I* __restrict__ row_ptrs, const I* __restrict__ col_idxs,
@@ -182,6 +192,7 @@ __global__ void __launch_bounds__(kSpmvThreads)
          row += (int64_t)gridDim.x * kRows) {
         const int64_t s = row_ptrs[row], e = row_ptrs[row + 1];
         V acc = V(0);
+        if (Epi::SUB && jv) acc = c[row * k + j] * V(-1);
         constexpr int kB = 4;
         for (int64_t t = s; t < e; t += kB) {
             I cc[kB];

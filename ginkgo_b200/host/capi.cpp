@@ -110,6 +110,8 @@ std::unique_ptr<LinOp> make_solver(std::shared_ptr<Executor> exec, int kind,
         auto f = solver::Minres<V>::build();
         // bit 6 of `fused`: the fused MINRES iteration is opt-in, as BiCGStab's and GMRES's
         f.with_criteria(crit).with_fused((fused & 64) != 0).with_check_every(check_every);
+        // bit 7: its iteration for 2..32 right-hand sides, opt-in and independent of bit 6
+        f.with_fused_multi_rhs((fused & 128) != 0);
         set_pre(f);
         return f.on(exec)->generate(A);
     }

@@ -127,6 +127,10 @@ struct viabi;
         static constexpr auto minres_fused_init = b200_minres_fused_init_##S;                   \
         static constexpr auto minres_fused_lanczos = b200_minres_fused_lanczos_##S;             \
         static constexpr auto minres_fused_update = b200_minres_fused_update_##S;               \
+        static constexpr auto minres_mrhs_work_size = b200_minres_mrhs_work_size_##S;           \
+        static constexpr auto minres_mrhs_init = b200_minres_mrhs_init_##S;                     \
+        static constexpr auto minres_mrhs_lanczos = b200_minres_mrhs_lanczos_##S;               \
+        static constexpr auto minres_mrhs_update = b200_minres_mrhs_update_##S;                 \
         static constexpr auto gmres_fused_work_size = b200_gmres_fused_work_size_##S;           \
         static constexpr auto gmres_fused_init = b200_gmres_fused_init_##S;                     \
         static constexpr auto gmres_fused_scale = b200_gmres_fused_scale_##S;                   \
@@ -167,6 +171,7 @@ GKOB_V(float, f32)
         static constexpr auto csr_spmv_dot2 = b200_csr_spmv_dot2_##S##_##T;                     \
         static constexpr auto csr_spmv_sub_dot = b200_csr_spmv_sub_dot_##S##_##T;               \
         static constexpr auto csr_spmv_mdot = b200_csr_spmv_mdot_##S##_##T;                     \
+        static constexpr auto csr_spmv_sub_mdot = b200_csr_spmv_sub_mdot_##S##_##T;             \
         static constexpr auto csr_spmv_mdot2 = b200_csr_spmv_mdot2_##S##_##T;                   \
         static constexpr auto csr_extract_diagonal = b200_csr_extract_diagonal_##S##_##T;       \
         static constexpr auto csr_convert_to_ell = b200_csr_convert_to_ell_##S##_##T;           \

@@ -1547,6 +1547,7 @@ class Minres : public SolverBase<V> {
 public:
     struct Factory : SolverFactoryBase<Factory> {
         bool fused_ = false;
+        bool fused_multi_rhs_ = false;
         int check_every_ = 16;
         // ginkgo_b200 extension: device-resident fused iteration where applicable (default off)
         Factory& with_fused(bool f)
@@ -1554,7 +1555,14 @@ public:
             fused_ = f;
             return *this;
         }
-        // iterations per graph launch (and per read of the control block) on the fused path
+        // ginkgo_b200 extension: the device-resident iteration for 2..32 right-hand sides, one
+        // matrix pass per iteration for all columns (opt-in, independent of with_fused)
+        Factory& with_fused_multi_rhs(bool f)
+        {
+            fused_multi_rhs_ = f;
+            return *this;
+        }
+        // iterations per graph launch (and per read of the control block) on the fused paths
         Factory& with_check_every(int k)
         {
             check_every_ = k;
@@ -1571,7 +1579,8 @@ public:
 
 protected:
     Minres(std::shared_ptr<const Executor> exec, const Factory& f, std::shared_ptr<const LinOp> op)
-        : Base(exec, f, op), fused_(f.fused_), check_every_(std::max(1, f.check_every_))
+        : Base(exec, f, op), fused_(f.fused_), fused_multi_rhs_(f.fused_multi_rhs_),
+          check_every_(std::max(1, f.check_every_))
     {}
     using Base::apply_impl;
     void apply_impl(const LinOp* lb, LinOp* lx) const override
@@ -1580,6 +1589,8 @@ protected:
         auto x = as<Dense>(lx);
         if (fused_ && try_fused<int32>(b, x)) return;
         if (fused_ && try_fused<int64>(b, x)) return;
+        if (fused_multi_rhs_ && try_fused_multi_rhs<int32>(b, x)) return;
+        if (fused_multi_rhs_ && try_fused_multi_rhs<int64>(b, x)) return;
         used_fused_ = false;
         auto exec = this->exec_;
         auto ctx = exec->ctx();
@@ -1697,12 +1708,81 @@ protected:
         return true;
     }
 
+    // Fused device-resident path for k = 2..32 right-hand sides (csrc/fused_minres_mrhs.cu): try_fused's
+    // admission with b and x of k columns stored without gaps, and its set-up on the n x k views.  Every
+    // column stops on its own; the device keeps a stopped column's scalars, x, p, q, v and z as the
+    // loop's masked steps leave them, and the host reads all k statuses at the end.
+    template <typename I>
+    bool try_fused_multi_rhs(const Dense* b, Dense* x) const
+    {
+        typename Base::template FusedProblem<I> f;
+        if (b->get_size().cols < 2 || !this->template fused_problem<I>(b, x, f, 32) ||
+            !this->template fused_scalar_preconditioner<I>(f) || f.res_kind == 1)
+            return false;
+        const auto A = f.A;
+        const V* inv_diag = f.inv_diag;
+        auto exec = this->exec_;
+        auto ctx = exec->ctx();
+        const int64 n = this->size_.rows;
+        const int64 k = (int64)b->get_size().cols;
+        const int64 nnz = A->get_num_stored_elements();
+        auto& m = mrhs_;
+        // workspace r, z, q, v, p0, p1 (n x k each), per-column scalars, statuses, control block, partials
+        m.reshape(n, k, [&] {
+            m.ws = Dense::create(exec, dim2{(size_type)(6 * n * k), 1});
+            m.sc = array<V>(exec, (size_type)(16 * k));
+            m.status = array<uint8>(exec, (size_type)k);
+            m.ctl = array<int32>(exec, 8);
+            m.work = array<V>(exec, (size_type)vabi<V>::minres_mrhs_work_size(ctx, k));
+        });
+        V* r = m.ws->get_values();
+        V *z = r + n * k, *q = r + 2 * n * k, *v = r + 3 * n * k, *p0 = r + 4 * n * k, *p1 = r + 5 * n * k;
+        V* xv = x->get_values();
+        V* sc = m.sc.get_data();
+        uint8* status = m.status.get_data();
+        int32* ctl = m.ctl.get_data();
+        V* work = m.work.get_data();
+        auto view = [&](V* d, int64 rows) {
+            return Dense::create_view(exec, dim2{(size_type)rows, (size_type)k}, d, (size_type)k);
+        };
+        auto rv = view(r, n), zv = view(z, n);
+        // the loop's set-up on k columns, its per-column scalars straight into slots sc[s k + .]
+        exec->copy(r, b->get_const_values(), n * k);
+        A->apply(this->neg_one_.get(), x, this->one_.get(), rv.get());
+        this->preconditioner_->apply(rv.get(), zv.get());
+        rv->compute_conj_dot(zv.get(), view(sc + k, 1).get());
+        zv->compute_conj_dot(zv.get(), view(sc + 6 * k, 1).get());
+        GKOB_CALL(vabi<V>::minres_initialize(ctx, n, k, r, k, z, k, p0, k, p1, k, q, k, v, k, v, k, sc + k,
+                                             sc + 2 * k, sc + 3 * k, sc + 9 * k, sc + 10 * k, sc + 11 * k,
+                                             sc + 12 * k, sc + 8 * k, sc + 7 * k, status));
+        if (f.baseline == 0) b->compute_norm2(view(sc + 4 * k, 1).get());
+        if (f.baseline == 1) rv->compute_norm2(view(sc + 4 * k, 1).get());
+        GKOB_CALL(vabi<V>::minres_mrhs_init(ctx, k, sc, status, ctl, f.max_iters, f.res_kind, f.iter_first,
+                                            f.baseline, (V)f.factor));
+        // the k-wide SpMV uses no plan
+        const FusedKey key{k, nnz, r, xv, {inv_diag}, A->get_const_row_ptrs(), A->get_const_col_idxs(),
+                           A->get_const_values()};
+        m.capture(ctx, key, 1, [&](int64) {
+            for (int it = 0; it < check_every_; ++it) {
+                GKOB_CALL((viabi<V, I>::csr_spmv_sub_mdot(ctx, n, n, nnz, A->get_const_row_ptrs(),
+                                                          A->get_const_col_idxs(), A->get_const_values(), z, k,
+                                                          v, sc, work, ctl)));
+                GKOB_CALL(vabi<V>::minres_mrhs_lanczos(ctx, n, k, v, q, inv_diag, sc, status, ctl, work));
+                GKOB_CALL(vabi<V>::minres_mrhs_update(ctx, n, k, xv, p0, p1, z, q, v, inv_diag, sc, status, ctl));
+            }
+        });
+        this->record(m.poll(*exec, "fused MINRES (several right-hand sides)", [] { return 0; }).second, m.status);
+        used_fused_ = true;
+        return true;
+    }
+
 private:
     using FusedKey = typename Base::FusedKey;
     bool fused_;
+    bool fused_multi_rhs_;
     int check_every_;
     mutable bool used_fused_ = false;
-    mutable typename Base::FusedState single_;
+    mutable typename Base::FusedState single_, mrhs_;
 };
 
 // ---------------------------------------------------------------------------------------------

@@ -761,6 +761,67 @@ B200_DECL_SPMV_SUB_DOT(f32, float, i32, int32_t)
 B200_DECL_SPMV_SUB_DOT(f32, float, i64, int64_t)
 
 /* ---------------------------------------------------------------------------
+ * Fused MINRES iteration for k = 2..32 right-hand sides (ginkgo_b200 extension behind
+ * solver::Minres::apply with with_fused_multi_rhs(true), single GPU).  The regrouping of the fused
+ * MINRES above with every vector n x k row-major (stride k) and every scalar per column; one matrix
+ * pass per iteration serves all columns.  minres::step_1 / step_2 of a stopped column are skipped, as
+ * the reference's kernels skip them by the column's stopping_status
+ * (reference/solver/minres_kernels.cpp:64-150); d = inv_diag of a scalar Jacobi preconditioner, NULL
+ * for Identity:
+ *   spmv_sub_mdot  v = A z - v for all columns, alpha_j = z_j . v_j in the SpMV epilogue
+ *                                     (Csr::apply(1, z, -1, v) with k columns + compute_conj_dot)
+ *   lanczos        v_j -= alpha_j q_j (also for alpha_j == 0, as sub_scaled with a 1 x k alpha);
+ *                  beta_j = v_j . (d v_j); then in the last CTA minres::step_1 of every running column
+ *                               (sub_scaled + jacobi apply + compute_conj_dot + minres::step_1)
+ *   update         minres::step_2 of every running column with z~ = d v recomputed and q_prev not
+ *                  stored; p / p_prev are p0 / p1 as the parity of the shared iteration count says
+ *                  (iteration i writes p1 when i is even, p0 when odd).  The last CTA swaps gamma /
+ *                  beta and runs the criterion check of the next iteration on every running column
+ *                  (std::swap(p, p_prev) + minres::step_2 + std::swap(gamma, beta) + criterion check)
+ *   init           the first criterion check of every column, after the host's minres::initialize
+ *                  with k columns; sc[4k + j] holds ||b_j|| (baseline 0) or ||r0_j|| (1) and is set to
+ *                  1 for baseline 2
+ * sc:     VT[16k]   sc[s*k + j]: s = 0 alpha, 1 beta, 2 gamma, 3 delta, 4 tau0, 5 threshold, 6 tau,
+ *                   7 eta, 8 eta_next, 9 cos_prev, 10 cos, 11 sin_prev, 12 sin
+ * status: uint8[k]  stopping_status byte of every column (0 = running)
+ * ctl:    int32[8]  0 nonzero once every column has stopped, 1 iterations, 2 max_iters (-1 none),
+ *                   3 res_kind (0 none, 2 ImplicitResidualNorm: sqrt|tau_j| <= threshold_j), 4 iter_first
+ * Once ctl[0] != 0 every kernel is a no-op, so graphs of several iterations can be replayed and the
+ * host polls ctl after each.  `work` has b200_minres_mrhs_work_size(k) elements.
+ *
+ * b200_csr_spmv_sub_mdot: c = A b - c for the k columns of the row-major b and c (stride k; square A,
+ * b also the dot operand) and dots[j] = b_j . c_j.  c is bit-identical to b200_csr_advanced_spmv with
+ * (alpha, beta) = (1, -1) and num_rhs = k; the dots are summed in a fixed order.  ctl may be NULL; with
+ * num_rows == 0 the dots are 0.  No plan and no alignment are required.
+ * ------------------------------------------------------------------------- */
+#define B200_DECL_FMINRESM(V, VT)                                                              \
+    int64_t b200_minres_mrhs_work_size_##V(const b200_ctx* ctx, int64_t k);                    \
+    b200_status b200_minres_mrhs_init_##V(b200_ctx* ctx, int64_t k, VT* sc, uint8_t* status,   \
+                                          int32_t* ctl, int64_t max_iters, int32_t res_kind,   \
+                                          int32_t iter_first, int32_t baseline,                \
+                                          VT reduction_factor);                                \
+    b200_status b200_minres_mrhs_lanczos_##V(b200_ctx* ctx, int64_t n, int64_t k, VT* v,       \
+                                             const VT* q, const VT* inv_diag, VT* sc,          \
+                                             const uint8_t* status, const int32_t* ctl,        \
+                                             VT* work);                                        \
+    b200_status b200_minres_mrhs_update_##V(b200_ctx* ctx, int64_t n, int64_t k, VT* x,        \
+                                            VT* p0, VT* p1, VT* z, VT* q, VT* v,               \
+                                            const VT* inv_diag, VT* sc, uint8_t* status,       \
+                                            int32_t* ctl);
+#define B200_DECL_SPMV_SUB_MDOT(V, VT, I, IT)                                                  \
+    b200_status b200_csr_spmv_sub_mdot_##V##_##I(                                              \
+        b200_ctx* ctx, int64_t num_rows, int64_t num_cols, int64_t nnz, const IT* row_ptrs,    \
+        const IT* col_idxs, const VT* values, const VT* b, int64_t k, VT* c, VT* dots,         \
+        VT* work, const int32_t* ctl);
+
+B200_DECL_FMINRESM(f64, double)
+B200_DECL_FMINRESM(f32, float)
+B200_DECL_SPMV_SUB_MDOT(f64, double, i32, int32_t)
+B200_DECL_SPMV_SUB_MDOT(f64, double, i64, int64_t)
+B200_DECL_SPMV_SUB_MDOT(f32, float, i32, int32_t)
+B200_DECL_SPMV_SUB_MDOT(f32, float, i64, int64_t)
+
+/* ---------------------------------------------------------------------------
  * Fused CG iteration for k = 2..32 right-hand sides (ginkgo_b200 extension behind solver::Cg::apply
  * with with_fused_multi_rhs(true), single GPU).  The regrouping of the fused CG above with every
  * vector n x k row-major (stride k) and every scalar per column; one matrix pass per iteration
